@@ -1,4 +1,4 @@
-"""Benchmark of the StyleTTS 2 text->waveform hot path on B200 (driver contract, see prompt section 4).
+"""Benchmark of the StyleTTS 2 text->waveform hot path on H100 (one JSON result line per run).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (default workload C2 per GPU)
     python bench.py --impl reference --steps K --warmup W    # the reference algorithm on host cores (oracle port)
@@ -56,7 +56,7 @@ def measured_peaks():
         d = json.load(open(p))
         return (float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), float(d["bf16_tflops"]),
                 "measured (MEASURED_PEAKS.json: copy GB/s, sustained cuBLAS bf16)")
-    return 6650.0, 1400.0, 1590.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet (dense bf16, HBM3), not a measurement"
 
 
 def ncu_traffic():
@@ -117,6 +117,25 @@ def make_inputs(wl, seed, pinned=False, B=None):
     if pinned:
         ts = [t.pin_memory() for t in ts]
     return ts
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write what the timed path returned in its last step as DIR/<name>.npy (float32).  An array larger than the budget
+    is replaced by a fixed, seeded sample of its elements (<name>.npy) plus the flat indices taken (<name>_index.npy)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget:
+            n = budget // 12                      # 4 bytes of value + 8 bytes of index per sampled element
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False)).astype(np.int64)
+            np.save(os.path.join(out_dir, f"{name}_index.npy"), idx)
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def kernel_family(name):
@@ -206,9 +225,11 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(args.steps):
-        step(devin)
+        wav_last = step(devin)
     e1.record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"wav": wav_last.view(B, L)})
     launches = lib.launch_count() - n0
     if args.graph:
         launches = graph_launches[0] * args.steps   # kernels of this library inside the replayed CUDA graph x replays
@@ -347,7 +368,7 @@ def run_ours(args):
         "config": {"workload": f"{args.workload}: {wl['desc']}", "per_gpu_batch": B, "global_batch": total_utts, "tokens": N, "frames": T,
                    "samples_per_utt": L, "diffusion_steps": wl["steps"],
                    "sharding": f"utterances over {world} rank(s) ({'one global batch split by shard_range' if args.global_batch else 'same batch per rank'}), no data-path collective",
-                   "l2": "inputs+activations per step (>3 GB) exceed the 126 MB L2; no flush needed",
+                   "l2": "inputs+activations per step (>3 GB) exceed the 50 MB L2; no flush needed",
                    "launch": "one CUDA graph per step" if args.graph else "eager"},
         "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "sync": "stream synchronise after every step's D2H copy"},
@@ -355,7 +376,7 @@ def run_ours(args):
         "per_rank_ms_per_step": per_rank_ms,
         "stages_ms": {k_: round(v_, 3) for k_, v_ in stage_ms.items()},
         "clocks": clk,
-        "roofline": {"kernel": "st2::tc::conv1d_tct_kernel (time-major, Cout <= 128) + st2::tc::conv1d_tc_kernel (channel-major, Cout >= 256): tcgen05 "
+        "roofline": {"kernel": "st2::tc::conv1d_tct_kernel (time-major, Cout <= 128) + st2::tc::conv1d_tc_kernel (channel-major, Cout >= 256): wgmma "
                                "implicit-GEMM Conv1d / polyphase ConvTranspose1d, fp16 high planes + e4m3 correction MMA, 2 MMA-times per fp32 "
                                "product; 3 in the F0/N predictor",
                      "bound": "tensor", "achieved": alg_tflops, "peak": tc_peak, "unit": "TFLOP/s", "frac": alg_tflops / tc_peak,
@@ -390,7 +411,7 @@ def run_ours(args):
 
 def cpu_reference(wl, sample_B, steps, warmup, probe=True):
     """The reference algorithm (oracle port, torch CPU fp32) on the host cores, bounded sample of the workload.
-    The imported reference itself (/root/reference) does not exist on the GPU box; the port is pinned against it
+    The port is pinned against the original implementation
     (tests/golden/PINNING*.json).  Thread count: a short probe at 8 / 32 / all cores picks the fastest."""
     sys.path.insert(0, os.path.join(ROOT, "oracle"))
     import styletts2_oracle as O
@@ -437,7 +458,7 @@ def cpu_reference(wl, sample_B, steps, warmup, probe=True):
             "thread_probe_samples_per_s": probe_res,
             "sample": f"{sample_B} utterance(s) of the workload ({wl['N']} tokens, {wl['N'] * wl['fpt']} frames, K={wl['steps']}), "
                       f"{warmup} warm-up + {len(ts)} timed runs (median), torch {torch.__version__} CPU, {best} of {ncpu} threads "
-                      f"(fastest of the probe); oracle port of the reference forward: /root/reference is not on the GPU box",
+                      f"(fastest of the probe); oracle port of the reference forward",
             "seconds_per_run": med, "runs_s": [round(t, 3) for t in ts]}
 
 
@@ -473,6 +494,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", dest="cpu_baseline", action="store_false")
     ap.add_argument("--no-graph", dest="graph", action="store_false", help="eager launches instead of one CUDA graph per step")
     ap.add_argument("--dump-launches", default=None, help="write the per-shape launch table (CUDA events, eager passes) to this JSON file")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the waveforms of the last timed step as DIR/<name>.npy (float32, at most 64 MB; seeded inputs)")
     ap.add_argument("--skip-e2e", action="store_true", help="profiling runs only (ncu): device-resident loop, no JSON contract line")
     args = ap.parse_args()
     if args.impl == "reference":

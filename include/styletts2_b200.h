@@ -1,4 +1,4 @@
-/* styletts2_b200 -- C ABI of the B200 (sm_100a) StyleTTS 2 inference hot path.
+/* styletts2_b200 -- C ABI of the H100 (sm_90a) StyleTTS 2 inference hot path.
  *
  * The reference (yl4579/StyleTTS2) is pure Python/PyTorch and has no FFI: the calls this
  * library replaces are the ATen operator calls inside the reference's nn.Module.forward
@@ -93,17 +93,17 @@ int st2_conv1d(const st2_conv_args* a, void* stream);
 /* number of stats partials st2_conv1d writes for Lq outputs */
 int st2_conv_stats_parts(int Lq);
 
-/* Tensor-core path of the same fused Conv1d (stride 1): tcgen05 implicit GEMM with TMEM accumulators,
+/* Tensor-core path of the same fused Conv1d (stride 1): wgmma implicit GEMM with register accumulators,
  * operands split into planes so that 16-bit / 8-bit tensor-core products reproduce the fp32 convolution (fp32
  * accumulate), weights streamed by 1-D TMA bulk copies.  `mode` selects the precision recipe (csrc/conv_tc.cu):
  *   ST2_TC_FAST      fp16 high planes + ONE e4m3 K=32 MMA carrying both correction terms: 2 MMA-times per product,
  *                    error ~2^-16 per product (vocoder / decoder convolutions; waveform bar 1e-3);
- *   ST2_TC_ACCURATE  two fp16 planes per operand, 3 MMAs, separate TMEM accumulator for the correction terms: error at
+ *   ST2_TC_ACCURATE  two fp16 planes per operand, 3 MMAs, separate accumulator for the correction terms: error at
  *                    the fp32-SIMT level (F0 / N predictor: F0 is integrated into a phase of 1e4..1e6 rad downstream);
  *   ST2_TC_F16X3     the accurate planes in a single accumulator (A/B testing).
  * `wtc` is the st2_conv_tc_weight_layout buffer (st2_conv_tc_weight_bytes bytes) built from the folded fp32 weight
  * [Cout,Cin,K] FOR THE SAME mode.  a->w is ignored; every other field means what it means for st2_conv1d,
- * except that it writes TWO statistics partials per 256-column tile (stats_nparts >= offset + 2*ceil(Lq/256)).
+ * except that it writes ONE statistics partial per 64-column tile (stats_nparts >= offset + ceil(Lq/64)).
  * x must live in an allocation whose first byte is 16-byte aligned (cudaMalloc / the PyTorch caching allocator):
  * rows are fetched as 16-byte copies of their aligned superset window.  Operand range: |z| < 1000 after the
  * prologue, |w| < 16 (fp16 planes of 64 z and 4096 w); larger values give inf/NaN loudly.
@@ -115,7 +115,7 @@ int st2_conv_stats_parts(int Lq);
  * (two M = 128 blocks per 256-frame tile), output channels on N = Cout rounded up to 32 (16 for Cout <= 16): no
  * tensor-pipe time or weight traffic for absent channels, epilogue stores straight from the accumulator registers (a warp
  * = 32 consecutive frames of one row), residual rows prefetched through a cp.async ring in shared memory, up to 8
- * accumulators in TMEM.  Layout and launch must use the same mode value.  Not with dup_q0_to >= 0.  (Cout = 256 as two
+ * accumulators in registers.  Layout and launch must use the same mode value.  Not with dup_q0_to >= 0.  (Cout = 256 as two
  * channel blocks was measured: no gain over the channel-major kernel and 3-16 % slower narrow layers from the extra tile
  * decode -- not kept.) */
 #define ST2_TC_TMAJOR 16
@@ -198,7 +198,7 @@ int st2_linear(const float* A, long long a_bs, long long a_ls, long long a_ks, i
                const float* bias, const float* R, long long ldr, float* C, long long ldc, int M, int Nf, int K,
                int act, void* stream);
 
-/* Tensor-core path of st2_linear for row-layout inputs (A element (m,k) at A + m*lda + k): tcgen05 GEMM with TMEM
+/* Tensor-core path of st2_linear for row-layout inputs (A element (m,k) at A + m*lda + k): wgmma GEMM with register
  * accumulators at fp32 accuracy -- operands split into three bf16 planes, six MMAs per product (the integer duration
  * boundary is downstream of the denoiser).  wtc from st2_linear_tc_weight_layout (st2_linear_tc_weight_bytes bytes),
  * built from the fp32 weight [Nf,K].  Same call sites as st2_linear. */
@@ -227,7 +227,7 @@ int st2_attention(const float* q, const float* kv, float* out, int B, int N, int
  * attention mask of transformers.AlbertModel (PL-BERT, Utils/PLBERT/util.py:6-12). */
 int st2_attention_ex(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out, long long out_ld,
                      const int* lengths, int B, int N, int H, int D, float scale, void* stream);
-/* The same contraction on the tensor cores (tcgen05, TMEM accumulators for S and O, fp16 two-plane split with separate
+/* The same contraction on the tensor cores (wgmma, register accumulators for S and O, fp16 two-plane split with separate
  * correction accumulators = fp32 accuracy; csrc/attention_tc.cu): one CTA per (128 query rows, head, utterance), keys in
  * blocks of 128.  Needs D == 64, row strides that are multiples of 4 floats and 16-byte aligned pointers
  * (st2_attention_tc_supported); arguments as st2_attention_ex. */

@@ -1,6 +1,6 @@
 """Pin the oracle against the UNMODIFIED reference and write tests/golden/ fixtures.
 
-Runs ONLY in the build container (needs /root/reference; see oracle/ref_import.py).
+Runs ONLY in the build container (needs the reference checkout ($STYLETTS2_REFERENCE); see oracle/ref_import.py).
     python oracle/make_golden.py
 
 For every case in oracle/cases.py it

@@ -1,4 +1,4 @@
-"""Fixtures for the notebook-level boundary (TEST INFRASTRUCTURE; build container only: needs /root/reference).
+"""Fixtures for the notebook-level boundary (TEST INFRASTRUCTURE; build container only: needs the reference checkout ($STYLETTS2_REFERENCE)).
 
 Writes, from the UNMODIFIED reference tree:
   tests/golden/textcleaner_vocab.json   the 178-entry symbol table of text_utils.py and the ids of three val_list rows
@@ -21,7 +21,7 @@ import yaml
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
-REF = os.environ.get("STYLETTS2_REFERENCE", "/root/reference")
+REF = os.environ.get("STYLETTS2_REFERENCE", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "..", "StyleTTS2"))
 GOLD = os.path.join(ROOT, "tests", "golden")
 
 

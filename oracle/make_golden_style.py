@@ -1,6 +1,6 @@
 """Pins oracle/style_oracle.py (SURVEY section 8 row f2) and writes tests/golden/style_libri.npz.
 
-BUILD CONTAINER ONLY (needs /root/reference and torchaudio).  Checks, on key-seeded weights and a seeded
+BUILD CONTAINER ONLY (needs the reference checkout ($STYLETTS2_REFERENCE) and torchaudio).  Checks, on key-seeded weights and a seeded
 synthetic clip:
   1. oracle log-mel  == torchaudio.transforms.MelSpectrogram pipeline of the notebooks (cell 5 `preprocess`)
   2. oracle StyleEncoder == the UNMODIFIED reference StyleEncoder (models.py:139-164), both encoders

@@ -1,6 +1,6 @@
 """Extra pinning of the oracle against the UNMODIFIED reference on configurations other than the committed fixtures
 (different seeds, batch sizes, token counts, sampler steps, guidance scales; both model families).  No fixtures are
-written -- only the measured agreement, to tests/golden/PINNING_SWEEP.json.  BUILD CONTAINER ONLY (needs /root/reference).
+written -- only the measured agreement, to tests/golden/PINNING_SWEEP.json.  BUILD CONTAINER ONLY (needs the reference checkout ($STYLETTS2_REFERENCE)).
 Run:  python -m oracle.pin_sweep
 """
 import json

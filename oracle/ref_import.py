@@ -1,7 +1,7 @@
-"""Import the UNMODIFIED reference (yl4579/StyleTTS2) read-only from /root/reference.
+"""Import the UNMODIFIED reference (yl4579/StyleTTS2) read-only from the reference checkout ($STYLETTS2_REFERENCE).
 
 TEST INFRASTRUCTURE ONLY.  Works only in the build container (the GPU box has no
-/root/reference); used by oracle/make_golden.py to pin the oracle restatement
+the reference checkout ($STYLETTS2_REFERENCE)); used by oracle/make_golden.py to pin the oracle restatement
 (oracle/styletts2_oracle.py) against the real reference forward and to emit the
 fixtures under tests/golden/.  Nothing in the product path imports this.
 
@@ -14,7 +14,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("STYLETTS2_REFERENCE", "/root/reference")
+REF_ROOT = os.environ.get("STYLETTS2_REFERENCE", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "..", "StyleTTS2"))
 
 
 def available() -> bool:

@@ -11,7 +11,7 @@ algorithm in yl4579/StyleTTS2 for the path SURVEY.md section 8(a) lists.  Every
 function cites the reference file:line it follows.  It is written from the
 reference's *behaviour*; it shares no class structure with it.
 
-Pinning: oracle/make_golden.py (build container only, where /root/reference is
+Pinning: oracle/make_golden.py (build container only, where the reference checkout ($STYLETTS2_REFERENCE) is
 mounted) runs the UNMODIFIED reference modules and this restatement on the
 same key-seeded weights and recorded RNG draws and asserts agreement
 (bit-exact for the integer durations, <=1e-5 for every float boundary; the

@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (libstyletts2_b200.so) in-tree with nvcc for sm_100a."""
+"""Build the C-ABI shared library (libstyletts2_b200.so) in-tree with nvcc for sm_90a (H100)."""
 from __future__ import annotations
 
 import glob
@@ -10,7 +10,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libstyletts2_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -43,7 +44,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [NVCC, "-shared", "-o", LIB, *objs, *ARCH, "-lcudart"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM) multi-head attention for the style denoiser and PL-BERT -- sm_100a.
+// Tensor-core (wgmma) multi-head attention for the style denoiser and PL-BERT -- sm_90a.
 //
 //   out[b, n, h, :] = softmax_m( scale * q[b,n,h,:] . k[b,m,h,:] ) v[b,m,h,:]        head dimension 64, N <= 4096 keys
 //   (Modules/diffusion/modules.py:523-535; transformers.AlbertModel's attention for PL-BERT, with a key-padding mask)
@@ -6,18 +6,17 @@
 // The predicted integer durations are downstream, so both contractions run at fp32 accuracy on the 16-bit tensor
 // cores with the recipe of linear_tc.cu: every operand is split into two fp16 planes, x = h + l * 2^-11 with h = fp16(x),
 // l = fp16((x - h) * 2^11); a product is h*h (accumulator MAIN) + h*l + l*h (accumulator CORR, 2^11 too large, folded in
-// by the reader with an exact 2^-11) -- three MMAs, two TMEM accumulators, so the small terms never get truncated
+// by the reader with an exact 2^-11) -- three MMAs, two register accumulators, so the small terms never get truncated
 // against the large running sum.
 //
-// One CTA = (128 query rows, one head, one utterance):
-//   S  = Q K^T   M = 128 queries, N = 128 keys per block, K = 64:  4 K-steps x 3 MMAs, accumulators S_main / S_corr
-//   P  = exp(scale * (S - rowmax))            one thread per query row = one TMEM lane: row max / row sum need no shuffles
-//   O += P V     M = 128 queries, N = 64 (d), K = 128 keys:        8 K-steps x 3 MMAs, accumulators O_main / O_corr
+// One CTA = one warpgroup = (64 query rows, one head, one utterance):
+//   S  = Q K^T   M = 64 queries, N = 128 keys per block, K = 64:  4 K-steps x 3 wgmmas, accumulators S_main / S_corr
+//   P  = exp(scale * (S - rowmax))            a row lives in the four lanes of a quad: row max / row sum need two shuffles
+//   O += P V     M = 64 queries, N = 64 (d), K = 128 keys:         8 K-steps x 3 wgmmas, accumulators O_main / O_corr
 // Keys are processed in blocks of 128.  With more than one block the row maxima are found in a first sweep over S (QK^T is
-// recomputed in the second sweep: cheap, and O never needs rescaling inside TMEM); N <= 128 takes a single sweep.
-// Operands are staged into the K-major no-swizzle ("interleave") UMMA layout by the row threads: Q / K / P as
+// recomputed in the second sweep: cheap, and O never needs rescaling); N <= 128 takes a single sweep.
+// Operands are staged into the K-major no-swizzle ("interleave") layout by the same threads: Q / K / P as
 // [k-chunk][row][8 x fp16], V transposed on the fly to [key-chunk][d][8 keys] (lanes run over d: coalesced global reads).
-// Warps 0-3: row workers (TMEM lane quarter = warp id), warp 4: TMEM allocation + single-thread MMA issue.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -30,19 +29,18 @@ namespace atc {
 
 using namespace st2::ptx;
 
-constexpr int QB = 128, KB = 128, HD = 64;
-constexpr int THREADS = 160;
+constexpr int QB = 64, KB = 128, HD = 64;
+constexpr int THREADS = 128;
 constexpr float LO_SCALE = 2048.0f, LO_UNSCALE = 1.0f / 2048.0f;
 constexpr int ROWS16 = 16;                                   // bytes per operand row chunk (8 fp16)
-constexpr int QK_LBO = QB * ROWS16;                          // 2048: distance between 8-wide k-chunks of Q / K / P
+constexpr int Q_LBO = QB * ROWS16;                           // 1024: distance between 8-wide k-chunks of Q and of P
+constexpr int K_LBO = KB * ROWS16;                           // 2048: distance between 8-wide k-chunks of K
 constexpr int V_LBO = HD * ROWS16;                           // 1024: distance between 8-key chunks of V^T
-constexpr int Q_PLANE = (HD / 8) * QK_LBO;                   // 16 KB
-constexpr int K_PLANE = (HD / 8) * QK_LBO;                   // 16 KB
+constexpr int Q_PLANE = (HD / 8) * Q_LBO;                    // 8 KB
+constexpr int K_PLANE = (HD / 8) * K_LBO;                    // 16 KB
 constexpr int V_PLANE = (KB / 8) * V_LBO;                    // 16 KB
-constexpr int P_PLANE = (KB / 8) * QK_LBO;                   // 32 KB
-constexpr int SM_Q = 0, SM_K = SM_Q + 2 * Q_PLANE, SM_V = SM_K + 2 * K_PLANE, SM_P = SM_V + 2 * V_PLANE, SM_BAR = SM_P + 2 * P_PLANE;
-constexpr int SM_TOTAL = SM_BAR + 64;
-constexpr int T_SMAIN = 0, T_SCORR = 128, T_OMAIN = 256, T_OCORR = 320, TMEM_COLS = 512;
+constexpr int P_PLANE = (KB / 8) * Q_LBO;                    // 16 KB
+constexpr int SM_Q = 0, SM_K = SM_Q + 2 * Q_PLANE, SM_V = SM_K + 2 * K_PLANE, SM_P = SM_V + 2 * V_PLANE, SM_TOTAL = SM_P + 2 * P_PLANE;
 
 struct Args {
   const float* q; long long q_ld;
@@ -53,13 +51,6 @@ struct Args {
   float scale;
 };
 
-__device__ __forceinline__ uint32_t idesc_f16(int n) {
-  uint32_t d = 0;
-  d |= 1u << 4;                       // D = F32, A = B = F16 (format 0), K-major
-  d |= (uint32_t)(n >> 3) << 17;
-  d |= (uint32_t)(128 >> 4) << 24;
-  return d;
-}
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& p0, uint32_t& p1) {
   const __half2 h = __floats2half2_rn(x0, x1);
   const float2 hf = __half22float2(h);
@@ -75,65 +66,51 @@ __device__ __forceinline__ void store_row8(uint8_t* plane0, int plane_bytes, siz
   *reinterpret_cast<uint4*>(plane0 + off) = make_uint4(a[0], a[1], a[2], a[3]);
   *reinterpret_cast<uint4*>(plane0 + plane_bytes + off) = make_uint4(b[0], b[1], b[2], b[3]);
 }
+__device__ __forceinline__ void load8(const float* p, float (&x)[8]) {
+  const float4 v0 = __ldg(reinterpret_cast<const float4*>(p)), v1 = __ldg(reinterpret_cast<const float4*>(p + 4));
+  x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
+}
 
 __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar_s = sbase + SM_BAR, bar_o = sbase + SM_BAR + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 16);
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
   const int N = a.N;
   const int klen = a.lengths ? min(a.lengths[b], N) : N;
   const int nkb = max(1, (klen + KB - 1) / KB);
-  if (tid == 0) {
-    mbar_init(bar_s, 1);
-    mbar_init(bar_o, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const bool worker = tid < QB;
-  const int row = qb * QB + tid;                    // query row of this worker == its TMEM lane
   const long long rowbase = (long long)b * N;
 
-  // ---- stage Q (once): worker t -> query row t, eight 8-wide chunks of d
-  if (worker) {
+  // ---- stage Q (once): thread t -> query row t % 64, four 8-wide chunks of d
+  {
+    const int r = tid & 63, row = qb * QB + r;
     const float* qr = a.q + (rowbase + min(row, N - 1)) * a.q_ld + h * HD;
 #pragma unroll
-    for (int c = 0; c < HD / 8; ++c) {
+    for (int c = (tid >> 6) * 4; c < (tid >> 6) * 4 + 4; ++c) {
       float x[8];
-      const float4 v0 = __ldg(reinterpret_cast<const float4*>(qr + 8 * c)), v1 = __ldg(reinterpret_cast<const float4*>(qr + 8 * c + 4));
-      x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
+      load8(qr + 8 * c, x);
       if (row >= N) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = 0.f;
       }
-      store_row8(smem + SM_Q, Q_PLANE, (size_t)c * QK_LBO + (size_t)tid * ROWS16, x);
+      store_row8(smem + SM_Q, Q_PLANE, (size_t)c * Q_LBO + (size_t)r * ROWS16, x);
     }
   }
-  auto stage_k = [&](int kb) {      // worker t -> key kb*128 + t
+  auto stage_k = [&](int kb) {      // thread t -> key kb*128 + t
     const int key = kb * KB + tid;
     const float* kr = a.k + (rowbase + min(key, N - 1)) * a.kv_ld + h * HD;
 #pragma unroll
     for (int c = 0; c < HD / 8; ++c) {
       float x[8];
-      const float4 v0 = __ldg(reinterpret_cast<const float4*>(kr + 8 * c)), v1 = __ldg(reinterpret_cast<const float4*>(kr + 8 * c + 4));
-      x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
+      load8(kr + 8 * c, x);
       if (key >= klen) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = 0.f;
       }
-      store_row8(smem + SM_K, K_PLANE, (size_t)c * QK_LBO + (size_t)tid * ROWS16, x);
+      store_row8(smem + SM_K, K_PLANE, (size_t)c * K_LBO + (size_t)tid * ROWS16, x);
     }
   };
-  auto stage_v = [&](int kb) {      // worker t -> d = t % 64, key chunks (t / 64) * 8 .. + 7; V^T rows of 8 keys
+  auto stage_v = [&](int kb) {      // thread t -> d = t % 64, key chunks (t / 64) * 8 .. + 7; V^T rows of 8 keys
     const int d = tid & 63, c0 = (tid >> 6) * 8;
 #pragma unroll 2
     for (int c = c0; c < c0 + 8; ++c) {
@@ -146,138 +123,118 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
       store_row8(smem + SM_V, V_PLANE, (size_t)c * V_LBO + (size_t)d * ROWS16, x);
     }
   };
-  auto issue_s = [&]() {            // S_main = Qh Kh^T ; S_corr = Qh Kl'^T + Ql' Kh^T
-    const uint32_t id = idesc_f16(KB);
+  float sm[64], sc[64];             // S fragment: row 16 w + g + 8 i, key 8 j + 2 t4 + c  ->  index 4 j + 2 i + c
+  auto compute_s = [&]() {          // S_main = Qh Kh^T ; S_corr = Qh Kl'^T + Ql' Kh^T
+    wg_fence();
 #pragma unroll
     for (int ks = 0; ks < HD / 16; ++ks) {
-      const uint32_t off = (uint32_t)ks * 2 * QK_LBO;
-      const uint64_t qh = make_desc(sbase + SM_Q + off, QK_LBO, 128), ql = make_desc(sbase + SM_Q + Q_PLANE + off, QK_LBO, 128);
-      const uint64_t kh = make_desc(sbase + SM_K + off, QK_LBO, 128), kl = make_desc(sbase + SM_K + K_PLANE + off, QK_LBO, 128);
-      tc_mma(tmem + T_SMAIN, qh, kh, id, ks ? 1u : 0u);
-      tc_mma(tmem + T_SCORR, qh, kl, id, ks ? 1u : 0u);
-      tc_mma(tmem + T_SCORR, ql, kh, id, 1u);
+      const uint64_t qh = make_desc(sbase + SM_Q + ks * 2 * Q_LBO, Q_LBO, 128), ql = make_desc(sbase + SM_Q + Q_PLANE + ks * 2 * Q_LBO, Q_LBO, 128);
+      const uint64_t kh = make_desc(sbase + SM_K + ks * 2 * K_LBO, K_LBO, 128), kl = make_desc(sbase + SM_K + K_PLANE + ks * 2 * K_LBO, K_LBO, 128);
+      wgmma_f16_n128(sm, qh, kh, ks ? 1u : 0u);
+      wgmma_f16_n128(sc, qh, kl, ks ? 1u : 0u);
+      wgmma_f16_n128(sc, ql, kh, 1u);
     }
-    tc_commit(bar_s);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(sm);
+    wg_fence_regs(sc);
+#pragma unroll
+    for (int r = 0; r < 64; ++r) sm[r] = fmaf(sc[r], LO_UNSCALE, sm[r]) * a.scale;
   };
-  auto issue_o = [&](bool first) {  // O_main += Ph Vh ; O_corr += Ph Vl' + Pl' Vh
-    const uint32_t id = idesc_f16(HD);
+  float om[32], oc[32];
+  auto compute_o = [&](bool first) {  // O_main += Ph Vh ; O_corr += Ph Vl' + Pl' Vh
+    wg_fence();
 #pragma unroll
     for (int ks = 0; ks < KB / 16; ++ks) {
-      const uint32_t po = (uint32_t)ks * 2 * QK_LBO, vo = (uint32_t)ks * 2 * V_LBO;
-      const uint64_t ph = make_desc(sbase + SM_P + po, QK_LBO, 128), pl = make_desc(sbase + SM_P + P_PLANE + po, QK_LBO, 128);
+      const uint32_t po = (uint32_t)ks * 2 * Q_LBO, vo = (uint32_t)ks * 2 * V_LBO;
+      const uint64_t ph = make_desc(sbase + SM_P + po, Q_LBO, 128), pl = make_desc(sbase + SM_P + P_PLANE + po, Q_LBO, 128);
       const uint64_t vh = make_desc(sbase + SM_V + vo, V_LBO, 128), vl = make_desc(sbase + SM_V + V_PLANE + vo, V_LBO, 128);
       const uint32_t acc = (first && ks == 0) ? 0u : 1u;
-      tc_mma(tmem + T_OMAIN, ph, vh, id, acc);
-      tc_mma(tmem + T_OCORR, ph, vl, id, acc);
-      tc_mma(tmem + T_OCORR, pl, vh, id, 1u);
+      wgmma_f16_n64(om, ph, vh, acc);
+      wgmma_f16_n64(oc, ph, vl, acc);
+      wgmma_f16_n64(oc, pl, vh, 1u);
     }
-    tc_commit(bar_o);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_regs(om);
+    wg_fence_regs(oc);
   };
-  const uint32_t lane_base = tmem + ((uint32_t)((warp & 3) * 32) << 16);
-  // S row of this worker, 32 columns at a time: s = scale * (main + corr * 2^-11)
-  auto read_s32 = [&](int c0, float (&s)[32]) {
-    float t[32];
-    tmem_ld32(lane_base + T_SMAIN + c0, s);
-    tmem_ld32(lane_base + T_SCORR + c0, t);
 #pragma unroll
-    for (int j = 0; j < 32; ++j) s[j] = fmaf(t[j], LO_UNSCALE, s[j]) * a.scale;
-  };
+  for (int r = 0; r < 32; ++r) { om[r] = 0.f; oc[r] = 0.f; }
 
-  uint32_t ph_s = 0, ph_o = 0;
-  float m = -INFINITY, l = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  auto row_max = [&](int kb) {
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+          if (kb * KB + 8 * j + 2 * t4 + c < klen) m[i] = fmaxf(m[i], sm[4 * j + 2 * i + c]);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      m[i] = fmaxf(m[i], __shfl_xor_sync(0xffffffffu, m[i], 1));
+      m[i] = fmaxf(m[i], __shfl_xor_sync(0xffffffffu, m[i], 2));
+    }
+  };
   const bool two_pass = nkb > 1;
   // ---- sweep 1 (only when there are several key blocks): row maxima
   if (two_pass) {
     for (int kb = 0; kb < nkb; ++kb) {
-      if (worker) stage_k(kb);
+      stage_k(kb);
       fence_proxy_async();
-      tc_fence_before();
       __syncthreads();
-      if (tid == QB) { tc_fence_after(); issue_s(); }
-      mbar_wait(bar_s, ph_s); ph_s ^= 1;
-      tc_fence_after();
-      if (worker) {
-#pragma unroll 1
-        for (int c0 = 0; c0 < KB; c0 += 32) {
-          float s[32];
-          read_s32(c0, s);
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (kb * KB + c0 + j < klen) m = fmaxf(m, s[j]);
-        }
-      }
-      tc_fence_before();
-      __syncthreads();       // S consumed, K buffer free (its MMAs have completed: bar_s)
+      compute_s();
+      row_max(kb);
+      __syncthreads();       // K buffer free
     }
   }
   // ---- sweep 2: P and O
   for (int kb = 0; kb < nkb; ++kb) {
-    if (kb > 0) { mbar_wait(bar_o, ph_o); ph_o ^= 1; }     // previous PV MMAs done: K / V / P buffers are free
-    if (worker) { stage_k(kb); stage_v(kb); }
+    stage_k(kb);
+    stage_v(kb);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    if (tid == QB) { tc_fence_after(); issue_s(); }
-    mbar_wait(bar_s, ph_s); ph_s ^= 1;
-    tc_fence_after();
-    if (worker) {
-      if (!two_pass) {
-#pragma unroll 1
-        for (int c0 = 0; c0 < KB; c0 += 32) {
-          float s[32];
-          read_s32(c0, s);
+    compute_s();
+    if (!two_pass) row_max(kb);
+    // P planes: this thread's two keys (8 j + 2 t4, + 1) of rows 16 w + g + 8 i -> 4 bytes of the row's 16-byte line in chunk j
 #pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (c0 + j < klen) m = fmaxf(m, s[j]);
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float p[2];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          p[c] = (kb * KB + 8 * j + 2 * t4 + c < klen) ? expf(sm[4 * j + 2 * i + c] - m[i]) : 0.f;
+          l[i] += p[c];
         }
+        uint32_t p0, p1;
+        split2(p[0], p[1], p0, p1);
+        const size_t off = (size_t)j * Q_LBO + (size_t)(16 * w + g + 8 * i) * ROWS16 + 4 * t4;
+        *reinterpret_cast<uint32_t*>(smem + SM_P + off) = p0;
+        *reinterpret_cast<uint32_t*>(smem + SM_P + P_PLANE + off) = p1;
       }
-#pragma unroll 1
-      for (int c0 = 0; c0 < KB; c0 += 32) {
-        float s[32];
-        read_s32(c0, s);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float p = (kb * KB + c0 + j < klen) ? expf(s[j] - m) : 0.f;
-          s[j] = p;
-          l += p;
-        }
-#pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          float x[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) x[j] = s[8 * cc + j];
-          store_row8(smem + SM_P, P_PLANE, (size_t)(c0 / 8 + cc) * QK_LBO + (size_t)tid * ROWS16, x);
-        }
-      }
-    }
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    if (tid == QB) { tc_fence_after(); issue_o(kb == 0); }
+    compute_o(kb == 0);
+    __syncthreads();         // K / V / P buffers free
   }
-  mbar_wait(bar_o, ph_o);
-  tc_fence_after();
-  if (worker) {     // tcgen05.ld is warp-collective: every lane of the worker warps runs the loads, only the stores are predicated
-    const float inv = 1.0f / l;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 1);
+    l[i] += __shfl_xor_sync(0xffffffffu, l[i], 2);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int row = qb * QB + 16 * w + g + 8 * i;
+    const float inv = 1.0f / l[i];
     float* orow = a.out + (rowbase + min(row, N - 1)) * a.out_ld + h * HD;
 #pragma unroll
-    for (int c0 = 0; c0 < HD; c0 += 32) {
-      float o[32], t[32];
-      tmem_ld32(lane_base + T_OMAIN + c0, o);
-      tmem_ld32(lane_base + T_OCORR + c0, t);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        float4 w;
-        w.x = fmaf(t[j], LO_UNSCALE, o[j]) * inv; w.y = fmaf(t[j + 1], LO_UNSCALE, o[j + 1]) * inv;
-        w.z = fmaf(t[j + 2], LO_UNSCALE, o[j + 2]) * inv; w.w = fmaf(t[j + 3], LO_UNSCALE, o[j + 3]) * inv;
-        if (row < N) *reinterpret_cast<float4*>(orow + c0 + j) = w;
-      }
+    for (int j = 0; j < 8; ++j) {
+      const int r = 4 * j + 2 * i;
+      const float2 o = make_float2(fmaf(oc[r], LO_UNSCALE, om[r]) * inv, fmaf(oc[r + 1], LO_UNSCALE, om[r + 1]) * inv);
+      if (row < N) *reinterpret_cast<float2*>(orow + 8 * j + 2 * t4) = o;
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(TMEM_COLS));
   }
 }
 

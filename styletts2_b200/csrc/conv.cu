@@ -2,7 +2,7 @@
 //
 //   y = epi( bias + sum_{ci,k} W * pre(x) )      -- see include/styletts2_b200.h
 //
-// Design (sm_100a, 148 SMs): one CTA = 256 threads computes a [CO_T x 256] output tile of one
+// Design (sm_90a, 132 SMs): one CTA = 256 threads computes a [CO_T x 256] output tile of one
 // utterance.  Lanes stride the time axis (conflict-free shared-memory reads of the staged frame
 // window for any dilation), warps stride output channels (weights are warp-broadcast 128-bit
 // loads).  The AdaIN affine + Snake/LeakyReLU prologue is applied ONCE while the window is staged

@@ -1,45 +1,42 @@
-// Tensor-core (tcgen05 / TMEM) implicit-GEMM Conv1d for the vocoder's AdaIN ResBlocks -- sm_100a.
+// Tensor-core (wgmma) implicit-GEMM Conv1d for the vocoder's AdaIN ResBlocks -- sm_90a.
 //
-//   D[co (M=128), t (N=256)] = sum_{tap} sum_{ci} W_tap[co, ci] * z[ci, t + tap*dil - pad],   z = snake/lrelu(a*x+b)
+//   D[co (M=128), t (N=64)] = sum_{tap} sum_{ci} W_tap[co, ci] * z[ci, t + tap*dil - pad],   z = snake/lrelu(a*x+b)
 //
 // Precision recipes (decided with the CPU oracle by emulation, DESIGN.md "precision"; tools/emulate_precision.py):
 // operands are pre-scaled by exact powers of two, w' = w * 2^12 and z' = z * 2^6 (the epilogue multiplies by 2^-18), so
 // that the fp16 "high" planes h = fp16(.) and the remainders l = (.) - h stay far away from fp16's subnormal range.
-//   ST2_TC_FAST  (vocoder / decoder, 2 MMA-times per product, double-buffered accumulator):
-//       D += h(w') h(z')                                   one kind::f16 MMA   (K = 16 channels)
-//          + [l(w')*2^4 | h(w')*2^-8] . [h(z')*2^-4 ; l(z')*2^8]   one kind::f8f6f4 MMA (e4m3, K = 32 = both corrections)
-//     the correction terms are 2^-11 of the leading one and e4m3 keeps 4 of their bits: ~15-16 operand bits in total,
-//     waveform error equal to the earlier bf16 hi/lo x3 recipe (emulated 3.9e-5 / 1.8e-4 vs 2.6e-5 / 1.1e-4 max-abs on the
-//     LJSpeech / LibriTTS decoder cases) at two thirds of its tensor-pipe time.  fp8 MMAs run at twice the fp16 rate, so
-//     the K=32 correction costs what one fp16 K=16 MMA costs.
+//   ST2_TC_FAST  (vocoder / decoder, 2 MMAs per product):
+//       D0 += h(w') h(z')                                   one f16 wgmma   (K = 16 channels)
+//       D1 += [l(w')*2^4 | h(w')*2^-8] . [h(z')*2^-4 ; l(z')*2^8]   one e4m3 wgmma (K = 32 = both corrections)
+//     the correction terms are 2^-11 of the leading one and e4m3 keeps 4 of their bits: ~15-16 operand bits in total.
+//     The e4m3 wgmma keeps fewer accumulator bits than the f16 one, so the corrections get their own accumulator
+//     (folded in by the epilogue): added into D0 they would round the large running sum.
 //   ST2_TC_ACCURATE (F0/N predictor: its F0 curve is integrated into a phase of 1e4..1e6 rad downstream):
-//       D0 += h(w') h(z');   D1 += h(w') l(z')*2^8 + l(w')*2^8 h(z')      three kind::f16 MMAs, TWO TMEM accumulators
+//       D0 += h(w') h(z');   D1 += h(w') l(z')*2^8 + l(w')*2^8 h(z')      three f16 wgmmas, TWO register accumulators
 //     (the tensor core truncates when it adds into an accumulator: keeping the small terms out of the big running sum
 //     brings the error to the fp32-SIMT level, see linear_tc.cu); the epilogue folds D1 in with an exact 2^-8.
-//     Both accumulators take 2 x 256 TMEM columns, so this mode is not double buffered (small layers only).
-//   ST2_TC_F16X3: the accurate planes accumulated into ONE double-buffered accumulator (3 MMAs; kept for A/B tests).
+//   ST2_TC_F16X3: the accurate planes accumulated into ONE accumulator (3 MMAs; kept for A/B tests).
 //
 // Mapping:
-//  * A operand = weights  [128 co x 16 ci], K-major, no-swizzle "interleave" layout (8-row x 16-byte core
-//    matrices, rows contiguous at 16 B pitch).  Pre-arranged in HBM so that one pipeline stage (tap, 16 ci,
-//    both planes) is ONE contiguous 8 KB block moved by a single 1-D TMA bulk copy (cp.async.bulk) that signals
-//    an mbarrier.
-//  * B operand = activations [256 t x 16 ci], K-major, same interleave layout: for each K chunk the frame window is a
+//  * A operand = weights  [64 co x 16 ci] per consumer warpgroup, K-major, no-swizzle "interleave" layout (8-row x 16-byte
+//    core matrices, rows contiguous at 16 B pitch).  Pre-arranged in HBM so that one pipeline stage (taps, 16 ci, both
+//    planes) is ONE contiguous block moved by a single 1-D TMA bulk copy (cp.async.bulk) that signals an mbarrier.
+//  * B operand = activations [64 t x 16 ci], K-major, same interleave layout: for each K chunk the frame window is a
 //    column of 16-byte rows, so a conv tap is just a descriptor start address shifted by tap*dil rows (16 B
 //    granularity) -- the window is staged ONCE per 16-channel block (AdaIN affine + Snake/LeakyReLU + plane split
 //    fused into the staging) and re-used by all K taps.
 //  * Raw fp32 frame windows travel HBM -> shared memory as 16-byte cp.async copies of the ALIGNED superset window of
 //    every channel row (rows of odd length start at any 4-byte phase; the phase becomes a per-channel offset of the
-//    scalar shared-memory reads of the conversion), four 20 KB blocks in flight per SM.
-//  * D accumulators live in TMEM (2 x 256 columns); the epilogue reads them with tcgen05.ld, transposes 32x32 blocks
-//    through shared memory for coalesced row stores and fuses bias, residual, MRF accumulation and the InstanceNorm
-//    partial statistics (count, mean, M2) exactly like the SIMT kernel.
-//  * Warp roles: warp 0 = TMEM alloc + single-thread MMA issue, warp 1 = weight TMA producer,
-//    warps 2-11 = activation stagers, warps 12-19 = epilogue.  Persistent CTAs (one per SM) loop over tiles.
+//    scalar shared-memory reads of the conversion), four blocks in flight per SM.
+//  * D accumulators live in the registers of two consumer warpgroups (output channels 0-63 / 64-127 of the tile); the
+//    epilogue works on the fragments and fuses bias, residual, MRF accumulation and the InstanceNorm partial statistics
+//    (count, mean, M2 per 64-frame tile) exactly like the SIMT kernel.
+//  * Warp roles: warps 0-7 = consumers (wgmma + epilogue), warp 8 = weight TMA producer, warps 9-18 = activation stagers.
+//    Persistent CTAs (one per SM) loop over tiles.
 //
 // TWO kernels share the stager and weight-producer roles (device functions below): the channel-major conv1d_tc_kernel
-// described above (Cout >= 256, ACCURATE / F16X3 recipes) and the TIME-MAJOR conv1d_tct_kernel further down (FAST recipe,
-// Cout <= 128: frames on the MMA's M axis, output channels on N; its header comment has the mapping).
+// described above and the TIME-MAJOR conv1d_tct_kernel further down (FAST recipe, Cout <= 128: frames on the MMA's M axis,
+// output channels on N; its header comment has the mapping).
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 
@@ -53,8 +50,8 @@ namespace tc {
 
 constexpr int MODE_FAST = ST2_TC_FAST, MODE_ACC = ST2_TC_ACCURATE, MODE_X3 = ST2_TC_F16X3;
 
-constexpr int TN = 256;
-constexpr int TM = 128;
+constexpr int TN = 64;                          // frames per tile (wgmma N of the channel-major kernel, M of the time-major one)
+constexpr int TM = 128;                         // output channels per tile of the channel-major kernel (two warpgroups of M = 64)
 constexpr int CB = 16;                          // input channels per pipeline block (one UMMA K step of the fp16 planes)
 constexpr int KCB = CB / 8;                     // 16-byte K chunks per plane and block
 constexpr int W_PLANE_BYTES = KCB * TM * 16;    // 4 KB
@@ -79,9 +76,9 @@ constexpr int CIN_PAD_MAX = 1120;
 constexpr int NUM_STAGERS = 320;                // 10 warps (8 would not buy registers: allocation is per 4 warps, 18 -> 20)
 constexpr int ST_PER_CH = NUM_STAGERS / CB;     // issue mapping: threads per channel row of a raw block
 constexpr int ROWS_PER_PASS = (NUM_STAGERS / 64) * 32;  // conversion mapping: rows covered per pass
-constexpr int NUM_EPI = 256;                    // 8 warps: two per TMEM lane quarter (each takes half of the columns)
-constexpr int THREADS = 64 + NUM_STAGERS + NUM_EPI;  // 640 = 20 warps (register allocation granularity: 4 warps)
-constexpr int TPITCH = 36;                      // epilogue transpose row pitch (floats), 16-byte aligned rows
+constexpr int NUM_CONS = 256;                   // two consumer warpgroups
+constexpr int ST0 = NUM_CONS + 32;              // first stager thread (warp 8 is the weight producer)
+constexpr int THREADS = ST0 + NUM_STAGERS;      // 608 = 19 warps
 
 // power-of-two operand scaling (exact): w' = w * 2^12, z' = z * 2^6; accumulators hold 2^18 x the convolution
 constexpr float W_SCALE = 4096.0f, X_SCALE = 64.0f, D_UNSCALE = 1.0f / (4096.0f * 64.0f);
@@ -93,65 +90,21 @@ constexpr int SM_ACT = SM_W + W_STAGES * W_STAGE_BYTES;
 constexpr int SM_RAW = SM_ACT + 2 * ACT_BUF_BYTES;
 constexpr int SM_COEF = SM_RAW + RAW_STAGES * RAW_BYTES;
 constexpr int SM_EPI = SM_COEF + 4 * CIN_PAD_MAX * 4;   // per-channel prologue coefficients of the current utterance (4 x 1120 floats)
-constexpr int SM_BAR = SM_EPI + 8 * (32 * TPITCH + 32) * 4;
+constexpr int SM_BAR = SM_EPI + 2 * 4 * 64 * 4;   // time-major statistics scratch [2 warpgroups][4 warps][64 channels]
 constexpr int SM_TOTAL = SM_BAR + 512;
 static_assert(RAW_CHUNKS % ST_PER_CH == 0 && NUM_STAGERS % 64 == 0, "stager mappings");
 static_assert(SM_TOTAL <= 232448, "shared memory budget (227 KB per CTA)");
 
 // barrier slots (8 B each) inside SM_BAR
-constexpr int B_WFULL = 0, B_WEMPTY = W_STAGES, B_AFULL = 2 * W_STAGES, B_AEMPTY = B_AFULL + 2, B_TFULL = B_AFULL + 4,
-              B_TEMPTY = B_AFULL + 6, B_COUNT = B_AFULL + 8;
+constexpr int B_WFULL = 0, B_WEMPTY = W_STAGES, B_AFULL = 2 * W_STAGES, B_AEMPTY = B_AFULL + 2, B_COUNT = B_AFULL + 4;
 static_assert(8 * B_COUNT + 8 <= 512, "barrier area");
 
-// Optional per-role cycle trace of CTA 0 (debug/profiling aid; null in production).
-__device__ long long* g_trace = nullptr;
 // Timing-experiment switches (tools/tc_bench.py; results are WRONG when any is set; 0 in production):
-//   1 = FAST recipe issues its second MMA as kind::f16 (cost of switching MMA kinds), 2 = epilogue without global traffic,
-//   4 = stagers skip the conversion (stale operands), 8 = no MMAs issued (commits only), 16 = no weight copies,
-//   32 = no raw activation copies, 64 = no epilogue at all
+//   4 = stagers skip the conversion (stale operands), 16 = no weight copies, 32 = no raw activation copies
 __device__ int g_dbg = 0;
-constexpr int TRACE_TILES = 16, TRACE_K = 8;  // [role 4][tile 16][8 counters]
-__device__ __forceinline__ void trace_put(int role, int it, int k, long long v) {
-  if (g_trace && blockIdx.x == 0 && it < TRACE_TILES) g_trace[(role * TRACE_TILES + it) * TRACE_K + k] = v;
-}
+__device__ long long* g_trace = nullptr;   // reserved for per-role cycle traces (st2_debug_set_trace); unused by these kernels
 
 using namespace st2::ptx;
-
-__device__ __forceinline__ long long mbar_wait_timed(uint32_t bar, uint32_t parity) {
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-  }
-  return clock64() - t0;
-}
-
-// Instruction descriptor: D = f32, A and B format code 0 (= F16 for kind::f16, = E4M3 for kind::f8f6f4), both K-major,
-// M = 128, N = 256.  The same bits serve both kinds.
-__device__ __forceinline__ uint32_t make_idesc() {
-  uint32_t d = 0;
-  d |= 1u << 4;                    // c_format = F32
-  d |= (uint32_t)(TN >> 3) << 17;  // n_dim
-  d |= (uint32_t)(TM >> 4) << 24;  // m_dim
-  return d;
-}
-__device__ __forceinline__ void tc_mma_f8(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f8f6f4 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Output channels of a 128-row tile are spread over the four TMEM lane quarters (an epilogue warp can only read the
-// quarter warp_id % 4): quarter q holds channels co0 + q*rq .. + rq-1 with rq = ceil(min(Cout - co0, 128) / 4).  For full
-// tiles rq = 32 (identity); for narrow layers (HiFi-GAN C = 64 / 32, conv_post) all eight epilogue warps get work.
-__host__ __device__ __forceinline__ int rows_per_quarter(int Cout, int cob) {
-  int rem = Cout - cob * TM;
-  if (rem > TM) rem = TM;
-  return (rem + 3) >> 2;
-}
 
 struct TileCoord {
   int b, cob, tq;
@@ -224,71 +177,7 @@ __device__ __forceinline__ void stage_row(const float (&x)[8], const float (&pa)
   }
 }
 
-// Epilogue row loop for one 32x32 accumulator block already transposed into T: row r of the block is output
-// channel (co_base + r); lane = column.  yp points at (row 0, this lane's column); rv[] holds the 32 residual
-// values of this lane's column (prefetched before the TMEM load so their latency is hidden).
-template <bool RES, int ACC, bool STATS, bool FULL>
-__device__ __forceinline__ void epi_rows(float* T, const float* bsm, float* yp, const float (&rv)[32], long long ystride,
-                                         int rmax, bool tv, int lane, float out_div, float acc_div) {
-  // FULL: all 32 rows and all 32 columns of the block are inside the tensor (warp-uniform): no predicates at all
-  const unsigned ys = (unsigned)ystride;
-#pragma unroll
-  for (int r0 = 0; r0 < 32; r0 += 8) {
-    if (FULL || r0 < rmax) {
-      float yo[8];
-      if (ACC) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) yo[i] = (FULL || (tv && (r0 + i) < rmax)) ? yp[(unsigned)(r0 + i) * ys] : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int r = r0 + i;
-        float val = T[r * TPITCH + lane] + bsm[r];
-        if (RES) val += rv[r];
-        if (out_div != 1.0f) val = __fdiv_rn(val, out_div);
-        if (ACC == 1) val = yo[i] + val;
-        if (ACC == 2) val = __fdiv_rn(yo[i] + val, acc_div);
-        if (FULL || (tv && r < rmax)) yp[(unsigned)r * ys] = val;
-        if (STATS) T[r * TPITCH + lane] = val;
-      }
-    }
-  }
-}
-
-// Vector variant for 16-byte aligned rows (row lengths multiples of 4 floats, unit output stride): lane -> (sub-row
-// lane / 8, column group lane % 8); pass p handles rows 4p .. 4p+3, each lane four consecutive columns: 128-bit shared
-// loads, 128-bit global loads / stores (a warp instruction moves four fully used 128-byte row segments) -- a quarter of
-// the memory instructions of the scalar path.  rv[4p + e] = residual of (row 4p + lane/8, column 4*(lane%8) + e).
-template <bool RES, int ACC, bool STATS>
-__device__ __forceinline__ void epi_rows_vec(float* T, const float* bsm, float* ybase, const float (&rv)[32], unsigned ys, int lane,
-                                             float out_div, float acc_div) {
-  const int sr = lane >> 3, cg = lane & 7;
-  float4 yo[8];
-  if (ACC) {
-#pragma unroll
-    for (int p = 0; p < 8; ++p) yo[p] = *reinterpret_cast<const float4*>(ybase + (unsigned)(4 * p + sr) * ys + 4 * cg);
-  }
-#pragma unroll
-  for (int p = 0; p < 8; ++p) {
-    const int r = 4 * p + sr;
-    float4 t4 = *reinterpret_cast<const float4*>(&T[r * TPITCH + 4 * cg]);
-    const float bb = bsm[r];
-    float val[4] = {t4.x + bb, t4.y + bb, t4.z + bb, t4.w + bb};
-    const float yv[4] = {ACC ? yo[p].x : 0.f, ACC ? yo[p].y : 0.f, ACC ? yo[p].z : 0.f, ACC ? yo[p].w : 0.f};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (RES) val[e] += rv[4 * p + e];
-      if (out_div != 1.0f) val[e] = __fdiv_rn(val[e], out_div);
-      if (ACC == 1) val[e] = yv[e] + val[e];
-      if (ACC == 2) val[e] = __fdiv_rn(yv[e] + val[e], acc_div);
-    }
-    const float4 o4 = make_float4(val[0], val[1], val[2], val[3]);
-    *reinterpret_cast<float4*>(ybase + (unsigned)r * ys + 4 * cg) = o4;
-    if (STATS) *reinterpret_cast<float4*>(&T[r * TPITCH + 4 * cg]) = o4;
-  }
-}
-
-// Weight producer role (one lane of warp 1): one 1-D TMA bulk copy per pipeline stage = up to `tps` consecutive taps of one
+// Weight producer role (one lane of warp 8): one 1-D TMA bulk copy per pipeline stage = up to `tps` consecutive taps of one
 // 16-channel block (contiguous in the [cob][cb][tap] layout), `wstep` bytes per (16 channels, tap) step.
 __device__ __forceinline__ void weight_producer_role(const uint4* __restrict__ wtc, const uint32_t sbase, const uint32_t bar0,
                                                      const int ncb, const int K, const int wstep, const int tps, const int stage_bytes,
@@ -317,7 +206,7 @@ __device__ __forceinline__ void weight_producer_role(const uint4* __restrict__ w
 }
 
 // ---------------------------------------------------------------------------------------------
-// Activation stager role (warps 2 .. 2 + NUM_STAGERS/32 - 1), shared by the channel-major and the time-major kernel: both
+// Activation stager role (warps ST0/32 .. ST0/32 + NUM_STAGERS/32 - 1), shared by the channel-major and the time-major kernel: both
 // read the staged window through the same K-major no-swizzle layout (one 16-byte row per frame and K chunk).
 template <int MODE>
 __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* smem, const uint32_t sbase, const uint32_t bar0,
@@ -332,7 +221,7 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
   // copies the 16-byte ALIGNED superset of its window; the phase (0..3 floats) is re-derived by the conversion.
   // Chunks outside the tensor are zero-filled (src-size 0), the chunk that crosses the end of the tensor is
   // trimmed; nothing before the 16-byte aligned start of the tensor's allocation is ever touched.
-  const int st = tid - 64;  // 0..319
+  const int st = tid - ST0;  // 0..319
   const int Lin_ = a.Lin, pre_act_ = a.pre_act, Cin_ = a.Cin;
   const float slope_ = a.pre_slope;
   const bool has_affine = a.pre_a != nullptr, is_snake = pre_act_ == ST2_ACT_SNAKE;
@@ -401,7 +290,7 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
   long long c_boff = 0;
   // conversion mapping: warp parity -> K chunk, (warp / 2, lane) -> ROWS_PER_PASS rows per pass: every shared-memory access of
   // a warp touches consecutive words / consecutive 16-byte rows
-  const int sw = warp - 2;
+  const int sw = warp - ST0 / 32;
   const int dbg_st = g_dbg;
   const int kc = sw & 1, rg = (sw >> 1) * 32 + lane;
   constexpr int NRC = (RW_MAX + ROWS_PER_PASS - 1) / ROWS_PER_PASS;
@@ -475,818 +364,393 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
   asm volatile("cp.async.wait_group 0;" ::: "memory");
 }
 
+// Release bookkeeping of the consumer warpgroups: the MMAs of one weight stage are committed as one wgmma group and at most
+// one group stays in flight, so a stage (and, after the last stage of a channel block, the activation buffer) is handed
+// back to its producer when the NEXT group has been issued and the wait leaves one pending.
+struct Pending {
+  int ws, as;   // weight stage of the group; activation buffer freed with it (-1: none)
+};
+__device__ __forceinline__ void release(const uint32_t bar0, const Pending& p, const bool leader) {
+  if (leader && p.ws >= 0) {
+    mbar_arrive(bar0 + 8u * (B_WEMPTY + p.ws));
+    if (p.as >= 0) mbar_arrive(bar0 + 8u * (B_AEMPTY + p.as));
+  }
+}
+
+// Output value of one element: bias, residual, divisor, MRF accumulation into y and output activation, in the order of the
+// SIMT kernel.  Returns the value written (the InstanceNorm statistics are taken of it).
+__device__ __forceinline__ float epi_value(const st2_conv_args& a, float v, float bias, const float* rrow, float* yp, int oidx) {
+  float val = v + bias;
+  if (rrow) val += rrow[oidx >> a.res_shift];
+  if (a.out_div != 1.0f) val = __fdiv_rn(val, a.out_div);
+  if (a.accum_mode == 1) val = yp[oidx] + val;
+  else if (a.accum_mode == 2) val = __fdiv_rn(yp[oidx] + val, a.accum_div);
+  if (a.out_act == ST2_ACT_TANH) val = tanhf(val);
+  yp[oidx] = val;
+  return val;
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
 conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int ncb, const int RW, const int ntiles,
                  const int n_tq, const int n_cob) {
   // RW = window rows (TN + (K-1)*dil, rounded up to 8); RWP = chunk pitch in rows
-  constexpr int NBUF = (MODE == MODE_ACC) ? 1 : 2;   // TMEM accumulator sets (ACCURATE needs both halves for one tile)
   const int RWP = RW + 2;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SM_BAR;
   auto BAR = [&](int i) { return bar0 + 8u * i; };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 8 * B_COUNT);
 
   if (tid == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 1); }
+    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
     for (int i = 0; i < 2; ++i) {
       mbar_init(BAR(B_AFULL + i), NUM_STAGERS);
-      mbar_init(BAR(B_AEMPTY + i), 1);
-      mbar_init(BAR(B_TFULL + i), 1);
-      mbar_init(BAR(B_TEMPTY + i), NUM_EPI);
+      mbar_init(BAR(B_AEMPTY + i), 2);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int K = a.K;
 
-  if (warp == 0) {
-    // ================================================================ MMA issuer
-    // Production path: the whole warp stays converged (every lane waits on the barriers), ONE elected lane issues the
-    // MMAs and commits; every quantity is warp-uniform, descriptors are (low, high) words and a tap only bumps the low
-    // word.  [A single lane walking the generic loop below spends ~250 cycles of dependent instructions per tap -- as
-    // long as the two MMAs of a tap take on the tensor pipe (profiles/r02_tc_bench_*.txt).]
-    if ((g_dbg & (1 | 8)) == 0 && !(g_trace != nullptr && blockIdx.x == 0)) {
-      const uint32_t idesc = make_idesc();
-      const uint32_t elected = elect_one();
-      const uint64_t da_d = make_desc(sbase + SM_W, TM * 16, 128), db_d = make_desc(sbase + SM_ACT, (uint32_t)RWP * 16, 128);
-      const uint32_t da_lo0 = (uint32_t)da_d, da_hi = (uint32_t)(da_d >> 32), db_lo0 = (uint32_t)db_d, db_hi = (uint32_t)(db_d >> 32);
-      const uint32_t dil_ = (uint32_t)a.dil;
-      int ws = 0, wph = 0, as = 0, aph = 0, it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int buf = it % NBUF;
-        mbar_wait(BAR(B_TEMPTY + buf), ((it / NBUF) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)buf * TN;
-        const uint32_t d1 = (MODE == MODE_ACC) ? tmem_base + TN : d0;
-        uint32_t acc = 0;
-        for (int cb = 0; cb < ncb; ++cb) {
-          mbar_wait(BAR(B_AFULL + as), aph);
-          tc_fence_after();
-          uint32_t b_lo = db_lo0 + (uint32_t)as * (ACT_BUF_BYTES >> 4);
-          for (int tap0 = 0; tap0 < K; tap0 += TPS) {
-            mbar_wait(BAR(B_WFULL + ws), wph);
-            tc_fence_after();
-            if (elected) {
-              uint32_t a_lo = da_lo0 + (uint32_t)ws * (W_STAGE_BYTES >> 4);
-              const int nt = min(TPS, K - tap0);
+  if (warp < NUM_CONS / 32) {
+    // ================================================================ consumers: wgmma (warpgroup wg = channels 64 wg ..) + epilogue
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+    const bool leader = (tid & 127) == 0;
+    const uint32_t lbo_a = TM * 16, lbo_b = (uint32_t)RWP * 16;
+    const uint32_t dil16 = (uint32_t)a.dil * 16u;
+    int ws = 0, wph = 0, as = 0, aph = 0;
+    Pending pend{-1, -1};
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const TileCoord tc_ = tile_coord(tile, n_tq, n_cob);
+      float d0[32], d1[32];
 #pragma unroll
-              for (int t = 0; t < TPS; ++t) {
-                if (t < nt) {
-                  if (MODE == MODE_FAST) {
-                    tc_mma_w(d0, a_lo, da_hi, b_lo, db_hi, idesc, acc);
-                    tc_mma_f8_w(d0, a_lo + (W_PLANE_BYTES >> 4), da_hi, b_lo + (ACT_PLANE_BYTES >> 4), db_hi, idesc, 1u);
-                  } else {
-                    tc_mma_w(d0, a_lo, da_hi, b_lo, db_hi, idesc, acc);
-                    tc_mma_w(d1, a_lo, da_hi, b_lo + (ACT_PLANE_BYTES >> 4), db_hi, idesc, MODE == MODE_ACC ? acc : 1u);
-                    tc_mma_w(d1, a_lo + (W_PLANE_BYTES >> 4), da_hi, b_lo, db_hi, idesc, 1u);
-                  }
-                  acc = 1;
-                  a_lo += W_STEP_BYTES >> 4;
-                  b_lo += dil_;
-                }
-              }
-              tc_commit(BAR(B_WEMPTY + ws));
-            } else {
-              acc = 1;
-              b_lo += dil_ * (uint32_t)min(TPS, K - tap0);
-            }
-            if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-          }
-          if (elected) tc_commit(BAR(B_AEMPTY + as));
-          if (++as == 2) { as = 0; aph ^= 1; }
-        }
-        if (elected) tc_commit(BAR(B_TFULL + buf));
-      }
-    } else if (lane == 0) {
-      const uint32_t idesc = make_idesc();
-      const uint32_t lbo_a = TM * 16, lbo_b = (uint32_t)RWP * 16;
-      const int dbg = g_dbg;
-      const uint64_t da_base = make_desc(sbase + SM_W, lbo_a, 128);
-      const int dil_ = a.dil;
-      int ws = 0, wph = 0, as = 0, aph = 0;
-      const bool tracing = (g_trace != nullptr) && blockIdx.x == 0;
-      auto wait_pumping = [&](uint32_t bar, uint32_t parity) -> long long {
-        if (tracing) return mbar_wait_timed(bar, parity);
-        mbar_wait(bar, parity);
-        return 0;
-      };
-      int it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int buf = it % NBUF;
-        const long long tt0 = tracing ? clock64() : 0;
-        long long w_te = wait_pumping(BAR(B_TEMPTY + buf), ((it / NBUF) & 1) ^ 1), w_af = 0, w_wf = 0;
-        tc_fence_after();
-        const uint32_t d0 = tmem_base + (uint32_t)buf * TN;
-        const uint32_t d1 = (MODE == MODE_ACC) ? tmem_base + TN : d0;
-        uint32_t first = 1;
-        for (int cb = 0; cb < ncb; ++cb) {
-          w_af += wait_pumping(BAR(B_AFULL + as), aph);
-          tc_fence_after();
-          // descriptors differ from stage to stage only in their 14-bit start-address field (address >> 4, bits 0-13)
-          const uint64_t db0_base = make_desc(sbase + SM_ACT + as * ACT_BUF_BYTES, lbo_b, 128);
-          for (int tap0 = 0; tap0 < K; tap0 += TPS) {
-            w_wf += wait_pumping(BAR(B_WFULL + ws), wph);
-            tc_fence_after();
-            const int nt = min(TPS, K - tap0);
-            for (int t = 0; t < nt; ++t) {
-              const uint64_t da0 = da_base + (uint64_t)(ws * (W_STAGE_BYTES >> 4) + t * (W_STEP_BYTES >> 4)), da1 = da0 + (W_PLANE_BYTES >> 4);
-              const uint64_t db0 = db0_base + (uint64_t)((tap0 + t) * dil_), db1 = db0 + (ACT_PLANE_BYTES >> 4);
-              if (dbg & 8) {
-              } else if (MODE == MODE_FAST) {
-                tc_mma(d0, da0, db0, idesc, first ? 0u : 1u);
-                if (dbg & 1) tc_mma(d0, da1, db1, idesc, 1u);
-                else tc_mma_f8(d0, da1, db1, idesc, 1u);         // both corrections in one e4m3 K=32 MMA
+      for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+      uint32_t acc = 0;
+      for (int cb = 0; cb < ncb; ++cb) {
+        mbar_wait(BAR(B_AFULL + as), aph);
+        uint32_t b_addr = sbase + SM_ACT + as * ACT_BUF_BYTES;
+        for (int tap0 = 0; tap0 < K; tap0 += TPS) {
+          mbar_wait(BAR(B_WFULL + ws), wph);
+          wg_fence();
+          uint32_t a_addr = sbase + SM_W + ws * W_STAGE_BYTES + wg * 64 * 16;
+          const int nt = min(TPS, K - tap0);
+#pragma unroll
+          for (int t = 0; t < TPS; ++t) {
+            if (t < nt) {
+              const uint64_t da0 = make_desc(a_addr, lbo_a, 128), da1 = make_desc(a_addr + W_PLANE_BYTES, lbo_a, 128);
+              const uint64_t db0 = make_desc(b_addr, lbo_b, 128), db1 = make_desc(b_addr + ACT_PLANE_BYTES, lbo_b, 128);
+              if (MODE == MODE_FAST) {
+                wgmma_f16_n64(d0, da0, db0, acc);
+                wgmma_e4m3_n64(d1, da1, db1, acc);     // both corrections in one e4m3 K=32 MMA, own accumulator
+              } else if (MODE == MODE_ACC) {
+                wgmma_f16_n64(d0, da0, db0, acc);
+                wgmma_f16_n64(d1, da0, db1, acc);
+                wgmma_f16_n64(d1, da1, db0, 1u);
               } else {
-                tc_mma(d0, da0, db0, idesc, first ? 0u : 1u);
-                tc_mma(d1, da0, db1, idesc, (MODE == MODE_ACC && first) ? 0u : 1u);
-                tc_mma(d1, da1, db0, idesc, 1u);
+                wgmma_f16_n64(d0, da0, db0, acc);
+                wgmma_f16_n64(d0, da0, db1, 1u);
+                wgmma_f16_n64(d0, da1, db0, 1u);
               }
-              first = 0;
+              acc = 1;
+              a_addr += W_STEP_BYTES;
+              b_addr += dil16;
             }
-            tc_commit(BAR(B_WEMPTY + ws));
-            if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
           }
-          tc_commit(BAR(B_AEMPTY + as));
-          if (++as == 2) { as = 0; aph ^= 1; }
+          wg_commit();
+          wg_wait<1>();
+          release(bar0, pend, leader);
+          pend.ws = ws;
+          pend.as = (tap0 + TPS >= K) ? as : -1;
+          if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
         }
-        tc_commit(BAR(B_TFULL + buf));
-        if (tracing) {
-          trace_put(0, it, 0, tt0); trace_put(0, it, 1, clock64()); trace_put(0, it, 2, w_te); trace_put(0, it, 3, w_af);
-          trace_put(0, it, 4, w_wf);
+        if (++as == 2) { as = 0; aph ^= 1; }
+      }
+      wg_wait<0>();
+      wg_fence_regs(d0);
+      if (MODE != MODE_X3) wg_fence_regs(d1);
+      release(bar0, pend, leader);
+      pend.ws = -1;
+
+      // ---- epilogue: row = output channel, column = frame
+      const int t0 = tc_.tq * TN;
+      const int ncols = min(TN, a.Lq - t0);
+      float* yb = a.y + (long long)tc_.b * a.y_bstride;
+      const float* rbase = a.res ? a.res + (long long)tc_.b * a.res_bstride : nullptr;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
+        const bool cok = co < a.Cout;
+        const float bias = (a.bias && cok) ? a.bias[co] : 0.f;
+        float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+        const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
+        float vals[16];
+        float s = 0.f, n = 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int r = 4 * j + 2 * i + c, col = 8 * j + 2 * t4 + c;
+            float v = d0[r];
+            if (MODE == MODE_ACC) v = fmaf(d1[r], ACC_LO_UNSCALE, v);
+            if (MODE == MODE_FAST) v += d1[r];
+            v *= D_UNSCALE;
+            float val = 0.f;
+            if (cok && col < ncols) {
+              val = epi_value(a, v, bias, rrow, yp, (t0 + col) * a.y_tstride + a.y_toffset);
+              s += val;
+              n += 1.f;
+            }
+            vals[2 * j + c] = val;
+            // ReflectionPad1d((1,0)) duplicate of the q==0 column (istftnet.py:365-366): value differs by its residual
+            if (col == 0 && t0 == 0 && a.dup_q0_to >= 0 && cok) {
+              const float dv = epi_value(a, v, bias, rrow, yp, a.dup_q0_to);
+              s += dv;   // one extra sample of this row
+              n += 1.f;
+            }
+          }
+        }
+        if (a.stats) {
+          // two-pass (count, mean, M2) of the row over the tile's frames: the four lanes t4 of a quad share the row
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+          n += __shfl_xor_sync(0xffffffffu, n, 1);
+          n += __shfl_xor_sync(0xffffffffu, n, 2);
+          const float mean = n > 0.f ? s / n : 0.f;
+          float m2 = 0.f;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int col = 8 * j + 2 * t4 + c;
+              const float dv = vals[2 * j + c] - mean;
+              if (col < ncols) m2 = fmaf(dv, dv, m2);
+            }
+          }
+          if (t0 == 0 && a.dup_q0_to >= 0 && t4 == 0 && cok) {
+            const float dv = yp[a.dup_q0_to] - mean;
+            m2 = fmaf(dv, dv, m2);
+          }
+          m2 += __shfl_xor_sync(0xffffffffu, m2, 1);
+          m2 += __shfl_xor_sync(0xffffffffu, m2, 2);
+          if (t4 == 0 && cok) {
+            float* sp = a.stats + (((long long)tc_.b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + tc_.tq) * 3;
+            sp[0] = n; sp[1] = mean; sp[2] = m2;
+          }
         }
       }
     }
-  } else if (warp == 1) {
+  } else if (warp == NUM_CONS / 32) {
     // ================================================================ weight producer (1-D TMA bulk copies)
     if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, W_STEP_BYTES, TPS, W_STAGE_BYTES, ntiles, n_tq, n_cob);
-  } else if (warp < 2 + NUM_STAGERS / 32) {
-    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
   } else {
-    // ================================================================ epilogue (8 warps)
-    const int ewi = warp - (2 + NUM_STAGERS / 32);  // 0..7
-    const int ew = warp & 3;                         // TMEM lane quarter this warp may access
-    const int half = ewi >> 2;                       // which 128 columns of the tile this warp handles
-    float* T = reinterpret_cast<float*>(smem + SM_EPI) + ewi * (32 * TPITCH + 32);
-    float* bsm = T + 32 * TPITCH;
-    const int y_len_ = a.y_len, res_len_ = a.res_len, acc_ = a.accum_mode, out_act_ = a.out_act, Cout_ = a.Cout, Lq_ = a.Lq;
-    const int ytst_ = a.y_tstride, ytoff_ = a.y_toffset, rshift_ = a.res_shift;
-    const float out_div_ = a.out_div, acc_div_ = a.accum_div;
-    const bool has_stats = a.stats != nullptr;
-    const bool dbg_noio = (g_dbg & 2) != 0;
-    // 128-bit epilogue path: every row of y / res starts 16-byte aligned and outputs are contiguous
-    const bool vec_ok = (ytst_ == 1) && (rshift_ == 0) && ((ytoff_ & 3) == 0) && ((y_len_ & 3) == 0) && ((a.y_bstride & 3) == 0) &&
-                        ((reinterpret_cast<size_t>(a.y) & 15) == 0) && (out_act_ == ST2_ACT_NONE) && (a.dup_q0_to < 0) &&
-                        (!a.res || (((res_len_ & 3) == 0) && ((a.res_bstride & 3) == 0) && ((reinterpret_cast<size_t>(a.res) & 15) == 0)));
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const TileCoord tc_ = tile_coord(tile, n_tq, n_cob);
-      const int buf = it % NBUF;
-      const int rq = rows_per_quarter(Cout_, tc_.cob);
-      const int co_base = tc_.cob * TM + ew * rq;
-      const int t0 = tc_.tq * TN;
-      const int ncols = min(TN, Lq_ - t0);
-      const int rmax = min(rq, Cout_ - co_base);  // warp-uniform (may be <= 0 for padded channel blocks)
-      bsm[lane] = (a.bias && lane < rmax) ? a.bias[co_base + lane] : 0.f;
-      float* yb = a.y + (long long)tc_.b * a.y_bstride + (long long)co_base * y_len_;
-      const float* rb = a.res ? a.res + (long long)tc_.b * a.res_bstride + (long long)co_base * res_len_ : nullptr;
-      // (L2 prefetches of the residual rows -- for this tile or one tile ahead -- were measured neutral / 12 % slower: the
-      // extra requests compete with the loads they are meant to help; profiles/r02_tc_bench_*.txt)
-      // Residual values of one 32x32 block: lane = column, rv[r] = row r.  The loads of block c+1 are issued right after
-      // the row loop of block c has consumed rv (same registers): their latency hides behind the statistics of block c
-      // and the TMEM load / transpose of block c+1; the first block's loads fly during the wait for the accumulator.
-      float rv[32];
-      auto load_rv = [&](int c0) {
-        const int tcol = t0 + c0 + lane;
-        const bool okc = (c0 + lane) < ncols;
-        const float* rp0 = rb ? rb + ((tcol * ytst_ + ytoff_) >> rshift_) : nullptr;
-        const unsigned rl = (unsigned)res_len_;
-        if (rb && vec_ok && rmax == 32 && (c0 + 32) <= ncols && !dbg_noio) {
-          const float* rq = rb + (t0 + c0 + ytoff_) + 4 * (lane & 7);
-#pragma unroll
-          for (int p = 0; p < 8; ++p) {
-            const float4 r4 = __ldg(reinterpret_cast<const float4*>(rq + (unsigned)(4 * p + (lane >> 3)) * rl));
-            rv[4 * p] = r4.x; rv[4 * p + 1] = r4.y; rv[4 * p + 2] = r4.z; rv[4 * p + 3] = r4.w;
-          }
-        } else if (rb && rmax == 32 && (c0 + 32) <= ncols && !dbg_noio) {
-#pragma unroll
-          for (int r = 0; r < 32; ++r) rv[r] = __ldg(rp0 + (unsigned)r * rl);
-        } else {
-#pragma unroll
-          for (int r = 0; r < 32; ++r) rv[r] = (rb && okc && r < rmax && !dbg_noio) ? __ldg(rp0 + (unsigned)r * rl) : 0.f;
-        }
-      };
-      load_rv(half * (TN / 2));
-      const long long ett0 = clock64();
-      const long long w_tf = mbar_wait_timed(BAR(B_TFULL + buf), (it / NBUF) & 1);
-      tc_fence_after();
-      if (g_dbg & 64) { tc_fence_before(); mbar_arrive(BAR(B_TEMPTY + buf)); continue; }   // timing experiment: no epilogue
-      float s_n = 0.f, s_mean = 0.f, s_m2 = 0.f;  // running (count, mean, M2) of row (co_base + lane)
-      long long tr_ld = 0, tr_st = 0, tr_ss = 0;
-      for (int c0 = half * (TN / 2); c0 < (half + 1) * (TN / 2); c0 += 32) {
-        float v[32];
-        const long long q0 = clock64();
-        const uint32_t taddr = tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(buf * TN + c0);
-        tmem_ld32(taddr, v);
-        if (MODE == MODE_ACC) {
-#pragma unroll
-          for (int hq = 0; hq < 2; ++hq) {
-            float vl[16];
-            tmem_ld16(taddr + TN + 16 * hq, vl);
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v[16 * hq + j] = fmaf(vl[j], ACC_LO_UNSCALE, v[16 * hq + j]);
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] *= D_UNSCALE;
-        const long long q1 = clock64();
-        tr_ld += q1 - q0;
-        if (c0 >= ncols || rmax <= 0 || dbg_noio) continue;
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(&T[lane * TPITCH + 4 * q]) = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        __syncwarp();
-        const int t = t0 + c0 + lane;
-        const bool tv = (c0 + lane) < ncols;
-        const int oidx = t * ytst_ + ytoff_;
-        const int ridx = oidx >> rshift_;
-        {
-          float* yp = yb + oidx;
-          const float* rp = rb ? rb + ridx : nullptr;
-          const long long ys = y_len_, rs = res_len_;
-          (void)rp; (void)rs;
-          if (out_act_ == ST2_ACT_NONE) {
-#define EPI_(RES_, ACC_, ST_, F_) epi_rows<RES_, ACC_, ST_, F_>(T, bsm, yp, rv, ys, rmax, tv, lane, out_div_, acc_div_)
-#define EPI(RES_, ACC_, ST_) do { if (full && vec_ok) epi_rows_vec<RES_, ACC_, ST_>(T, bsm, yb + (t0 + c0 + ytoff_), rv, (unsigned)ys, lane, out_div_, acc_div_); \
-                                 else if (full) EPI_(RES_, ACC_, ST_, true); else EPI_(RES_, ACC_, ST_, false); } while (0)
-            const bool full = (rmax == 32) && (ncols - c0 >= 32);
-            if (has_stats) {
-              if (rb) { if (acc_ == 0) EPI(true, 0, true); else if (acc_ == 1) EPI(true, 1, true); else EPI(true, 2, true); }
-              else    { if (acc_ == 0) EPI(false, 0, true); else if (acc_ == 1) EPI(false, 1, true); else EPI(false, 2, true); }
-            } else {
-              if (rb) { if (acc_ == 0) EPI(true, 0, false); else if (acc_ == 1) EPI(true, 1, false); else EPI(true, 2, false); }
-              else    { if (acc_ == 0) EPI(false, 0, false); else if (acc_ == 1) EPI(false, 1, false); else EPI(false, 2, false); }
-            }
-#undef EPI_
-#undef EPI
-          } else {  // rare generic path (output activation)
-            for (int r = 0; r < rmax; ++r) {
-              float val = 0.f;
-              if (tv) {
-                val = T[r * TPITCH + lane] + bsm[r];
-                if (rb) val += rv[r];
-                if (out_div_ != 1.0f) val = __fdiv_rn(val, out_div_);
-                if (acc_ == 1) val = yp[(long long)r * ys] + val;
-                else if (acc_ == 2) val = __fdiv_rn(yp[(long long)r * ys] + val, acc_div_);
-                if (out_act_ == ST2_ACT_TANH) val = tanhf(val);
-                yp[(long long)r * ys] = val;
-              }
-              if (has_stats) T[r * TPITCH + lane] = val;
-            }
-          }
-        }
-        if (c0 + 32 < (half + 1) * (TN / 2)) load_rv(c0 + 32);
-        const long long q2 = clock64();
-        tr_st += q2 - q1;
-        // ReflectionPad1d((1,0)) duplicate of the q==0 column (istftnet.py:365-366): value differs by its residual
-        const bool dup_here = (a.dup_q0_to >= 0) && (t0 == 0) && (c0 == 0);
-        float dupv = 0.f;
-        if (dup_here && lane < rmax) {
-          float val = v[0] + bsm[lane];
-          if (rb) val += rb[(long long)lane * a.res_len + (a.dup_q0_to >> a.res_shift)];
-          if (a.out_div != 1.0f) val = __fdiv_rn(val, a.out_div);
-          float* p = yb + (long long)lane * a.y_len + a.dup_q0_to;
-          if (a.accum_mode == 1) val = *p + val;
-          else if (a.accum_mode == 2) val = __fdiv_rn(*p + val, a.accum_div);
-          if (a.out_act == ST2_ACT_TANH) val = tanhf(val);
-          *p = val;
-          dupv = val;
-        }
-        if (has_stats) {
-          __syncwarp();
-          const int nv = min(32, ncols - c0);
-          float w[32];
-#pragma unroll
-          for (int q = 0; q < 8; ++q) {
-            const float4 t4 = *reinterpret_cast<const float4*>(&T[lane * TPITCH + 4 * q]);
-            w[4 * q] = t4.x; w[4 * q + 1] = t4.y; w[4 * q + 2] = t4.z; w[4 * q + 3] = t4.w;
-          }
-          float cs = 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) cs += (j < nv) ? w[j] : 0.f;
-          const float cmean = cs / (float)nv;
-          float cm2 = 0.f;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            const float d = (j < nv) ? w[j] - cmean : 0.f;
-            cm2 = fmaf(d, d, cm2);
-          }
-          const float nn = s_n + (float)nv;  // Chan merge
-          const float delta = cmean - s_mean;
-          s_mean += delta * ((float)nv / nn);
-          s_m2 += cm2 + delta * delta * (s_n * (float)nv / nn);
-          s_n = nn;
-          if (dup_here) {  // one extra sample for this row
-            const float n2 = s_n + 1.0f;
-            const float d2 = dupv - s_mean;
-            s_mean += d2 / n2;
-            s_m2 += d2 * d2 * (s_n / n2);
-            s_n = n2;
-          }
-        }
-        __syncwarp();
-        tr_ss += clock64() - q2;
-      }
-      tc_fence_before();
-      mbar_arrive(BAR(B_TEMPTY + buf));
-      if (ewi == 0 && lane == 0) {
-        trace_put(3, it, 0, ett0); trace_put(3, it, 1, clock64()); trace_put(3, it, 2, w_tf);
-        trace_put(3, it, 3, tr_ld); trace_put(3, it, 4, tr_st); trace_put(3, it, 5, tr_ss);
-      }
-      if (a.stats && lane < rmax) {
-        float* sp = a.stats + (((long long)tc_.b * a.Cout + co_base + lane) * a.stats_nparts + a.stats_part_offset + 2 * tc_.tq + half) * 3;
-        sp[0] = s_n; sp[1] = s_mean; sp[2] = s_m2;
-      }
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
   }
 }
 
 // =============================================================================================
 // TIME-MAJOR variant for narrow layers (Cout <= 128; HiFi-GAN C = 64 / 32 stages, conv_post): the operand roles are
 // swapped --
-//     D[t (M = 128 per MMA, two M blocks per 256-frame tile), co (N = NC)] = sum_tap sum_ci z[ci, t + tap*dil - pad] * W_tap[co, ci]
-// The staged activation window is the A operand (same K-major 16-byte-row layout, a tap is still a descriptor shift, M block
-// 1 is the window advanced by 128 rows), the weights are the B operand with only NC = Cout rounded up to 32 (16 for
-// Cout <= 16) rows: no tensor-pipe time and no weight traffic is spent on absent output channels (the channel-major kernel
-// runs M = 128 for Cout = 32).  In TMEM a lane is a FRAME and a column is a channel, so an epilogue thread owns one frame
-// of every channel: a warp's store of one accumulator register is 128 contiguous bytes of one output row -- no transpose
-// through shared memory.  The InstanceNorm partials are reduced across the warp's 32 frames with a transposing shuffle tree
-// (62 shuffles per 32 channels for the sum and the sum of squares of the deviation from a pilot sample), the four warps of an
-// M block merge their (count, mean, M2) records through shared memory in fixed order: two partials per tile like the
-// channel-major kernel.  FAST recipe only.
+//     D[t (M = 64 frames per tile), co (N = NC / 2 per warpgroup)] = sum_tap sum_ci z[ci, t + tap*dil - pad] * W_tap[co, ci]
+// The staged activation window is the A operand (same K-major 16-byte-row layout, a tap is still a descriptor shift), the
+// weights are the B operand with only NC = Cout rounded up to 32 (16 for Cout <= 16) rows: no tensor-pipe time and no weight
+// traffic is spent on absent output channels.  The two consumer warpgroups take one half of the channels each.  The
+// InstanceNorm partials of a channel are reduced over the warp's 16 frames with shuffles and over the four warps of a
+// warpgroup through shared memory (two passes: mean, then M2).  FAST recipe only.
 __host__ __device__ __forceinline__ int tmajor_nc(int Cout) { return Cout <= 16 ? 16 : ((Cout + 31) & ~31); }
 
-// Shared memory of the time-major kernel: the weight ring uses 8 KB stages (the first half of the channel-major ring), the
-// second half and whatever the statistics scratch ([2 tile parities][8 warps][NC][3] floats) leaves of the epilogue area hold
-// the RESIDUAL RING: 2 KB slots (16 channels x 32 frames) filled by 4-byte cp.async copies, up to three steps ahead per warp.
 constexpr int T_WSTAGE = 8192;                            // bytes per weight stage: 8 taps (NC = 16) .. 1 tap (NC = 128)
-constexpr int SM_TRES_A = SM_W + W_STAGES * T_WSTAGE;     // 12 residual slots in the unused half of the weight ring
-constexpr int T_SLOT = 2048, T_SLOTS_A = (W_STAGES * (W_STAGE_BYTES - T_WSTAGE)) / T_SLOT;
-constexpr int SM_TBIAS = SM_EPI;                          // 128 floats
-constexpr int SM_TPILOT = SM_TBIAS + 512;                 // [8 warps][32] floats
-constexpr int SM_TSTAT = SM_TPILOT + 8 * 32 * 4;          // [2][8][NC][3] floats, then residual slots up to SM_BAR
-static_assert(SM_TSTAT + 2 * 8 * 128 * 3 * 4 <= SM_BAR, "time-major epilogue scratch");
-static_assert(T_SLOTS_A + (SM_BAR - SM_TSTAT - 2 * 8 * 128 * 3 * 4) / T_SLOT >= 16, "two residual steps per warp in flight for NC = 128");
 
-template <bool RES, int ACC>
-__device__ __forceinline__ void tct_rows(float (&v)[16], const float (&rv)[16], const float* bsm_c0, float* yp0, const unsigned ys,
-                                         const int nch, const bool tv, const float out_div, const float acc_div, const int out_act) {
-#pragma unroll
-  for (int j0 = 0; j0 < 16; j0 += 8) {
-    if (j0 < nch) {   // warp-uniform
-      float yo[8];
-      if (ACC) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) yo[i] = (tv && (j0 + i) < nch) ? yp0[(unsigned)(j0 + i) * ys] : 0.f;
-      }
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int j = j0 + i;
-        float val = v[j] * D_UNSCALE + bsm_c0[j];
-        if (RES) val += rv[j];
-        if (out_div != 1.0f) val = __fdiv_rn(val, out_div);
-        if (ACC == 1) val = yo[i] + val;
-        if (ACC == 2) val = __fdiv_rn(yo[i] + val, acc_div);
-        if (out_act == ST2_ACT_TANH) val = tanhf(val);
-        const bool ok = tv && j < nch;
-        if (ok) yp0[(unsigned)j * ys] = val;
-        v[j] = ok ? val : 0.f;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) v[j0 + i] = 0.f;
-    }
-  }
+template <int NH>   // channels per warpgroup = NC / 2
+__device__ __forceinline__ void tct_mma(float (&d)[NH / 2], float (&e)[NH / 2], uint64_t a0, uint64_t b0, uint64_t a1, uint64_t b1,
+                                        uint32_t acc) {
+  if constexpr (NH == 8) { wgmma_f16_n8(d, a0, b0, acc); wgmma_e4m3_n8(e, a1, b1, acc); }
+  else if constexpr (NH == 16) { wgmma_f16_n16(d, a0, b0, acc); wgmma_e4m3_n16(e, a1, b1, acc); }
+  else if constexpr (NH == 32) { wgmma_f16_n32(d, a0, b0, acc); wgmma_e4m3_n32(e, a1, b1, acc); }
+  else if constexpr (NH == 48) { wgmma_f16_n48(d, a0, b0, acc); wgmma_e4m3_n48(e, a1, b1, acc); }
+  else { wgmma_f16_n64(d, a0, b0, acc); wgmma_e4m3_n64(e, a1, b1, acc); }
 }
 
-// Full step (16 existing channels, 32 existing frames, plain epilogue): no predicates, the output pointer advances row by row.
-// yo = the 16 values of y to accumulate into (ACC != 0), loaded one step ahead by the caller.
-template <bool RES, int ACC>
-__device__ __forceinline__ void tct_rows_full(float (&v)[16], const float (&rv)[16], const float (&yo)[16], const float* bsm_c0, float* yp0,
-                                              const unsigned ys, const float acc_div) {
-  float bb[16];
-#pragma unroll
-  for (int k4 = 0; k4 < 4; ++k4) {
-    const float4 b4 = *reinterpret_cast<const float4*>(bsm_c0 + 4 * k4);
-    bb[4 * k4] = b4.x; bb[4 * k4 + 1] = b4.y; bb[4 * k4 + 2] = b4.z; bb[4 * k4 + 3] = b4.w;
-  }
-  float* p = yp0;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    float val = v[j] * D_UNSCALE + bb[j];
-    if (RES) val += rv[j];
-    if (ACC == 1) val = yo[j] + val;
-    if (ACC == 2) val = __fdiv_rn(yo[j] + val, acc_div);
-    *p = val;
-    v[j] = val;
-    p += ys;
-  }
-}
-
-// One step of the transposing reduction: 2N values per lane -> N values per lane, each summed with the partner lane (lane ^ N).
-template <int N>
-__device__ __forceinline__ void xreduce_step(float* d, const int lane) {
-  const bool up = (lane & N) != 0;
-#pragma unroll
-  for (int i = 0; i < N; ++i) {
-    const float send = up ? d[i] : d[i + N];
-    const float keep = up ? d[i + N] : d[i];
-    d[i] = keep + __shfl_xor_sync(0xffffffffu, send, N);
-  }
-}
-
-constexpr int T_TFULL = 16, T_TEMPTY = 24, T_MAXBUF = 8;   // barrier slots of the accumulator ring (time-major kernel)
-
-// Epilogue role of the time-major kernel.  HAS_ACC: the launch accumulates into y (MRF sum, accum_mode != 0): the y values of a
-// full step are loaded one step ahead into registers (a read at the point of use would expose the HBM latency 16 times per step).
-template <bool HAS_ACC>
-__device__ __forceinline__ void tct_epilogue_role(const st2_conv_args& a, uint8_t* smem, const uint32_t sbase, const uint32_t bar0,
-                                                  const uint32_t tmem_base, const int ntiles, const int n_tq, const int NC, const int NBUF,
-                                                  const int tid, const int warp, const int lane) {
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-  // ================================================================ epilogue (8 warps): warp -> (M block, 32 frames)
-  // The work of a warp is the sequence of (tile, 16-channel group) steps of its frames.  The residual values of a step
-  // travel HBM -> shared memory as 4-byte cp.async copies (each lane copies and later reads its own frame of 16 rows: one
-  // 128-byte row piece per warp instruction, no registers held while in flight) issued D = 2 or 3 steps ahead -- across
-  // tile boundaries -- so 32-48 KB of residual rows are in flight per SM while the accumulator ring lets the MMAs run ahead.
-  // A ring slot is [16 channels][32 frames] floats with the 16-byte chunks of a row XOR-swizzled by (channel & 7): the
-  // finished values of a step go back into the slot the residuals came from (same word per lane), and the InstanceNorm
-  // partials read it TRANSPOSED -- lane = (channel, half of the frames), four conflict-free 128-bit loads.
-  const int ewi = warp - (2 + NUM_STAGERS / 32);  // 0..7
-  const int q = warp & 3;                          // TMEM lane quarter this warp may access = frames 32q .. 32q+31 of the M block
-  const int m = ewi >> 2;                          // M block (which 128 frames of the tile)
-  const int et = tid - (64 + NUM_STAGERS);         // 0..255
-  float* sstat = reinterpret_cast<float*>(smem + SM_TSTAT);
-  float* bsm = reinterpret_cast<float*>(smem + SM_TBIAS);
-  float* pil = reinterpret_cast<float*>(smem + SM_TPILOT) + ewi * 32;
-  const int y_len_ = a.y_len, res_len_ = a.res_len, acc_ = a.accum_mode, out_act_ = a.out_act, Cout_ = a.Cout, Lq_ = a.Lq;
-  const int ytst_ = a.y_tstride, ytoff_ = a.y_toffset, rshift_ = a.res_shift;
-  const float out_div_ = a.out_div, acc_div_ = a.accum_div;
-  const bool has_stats = a.stats != nullptr, has_res = a.res != nullptr;
-  const bool plain = (out_div_ == 1.0f) && (out_act_ == ST2_ACT_NONE);
-  const int ng = NC >> 4;                          // 16-channel groups per tile
-  const int fr0 = m * 128 + q * 32;                // first frame of this warp within a tile
-  const int tl = fr0 + lane;                       // this lane's frame within a tile
-  // residual ring: slots 0 .. T_SLOTS_A-1 behind the weight ring, the others behind the statistics scratch
-  const int res_b0 = SM_TSTAT + 2 * 8 * NC * 3 * 4;
-  const int D = min(3, (T_SLOTS_A + (SM_BAR - res_b0) / T_SLOT) / 8);      // steps ahead (>= 2, see static_assert)
-  auto slot_base = [&](int p) -> uint32_t {
-    const int k = p * 8 + ewi;
-    return sbase + (uint32_t)(k < T_SLOTS_A ? SM_TRES_A + k * T_SLOT : res_b0 + (k - T_SLOTS_A) * T_SLOT);
-  };
-  // byte offset of (channel j, this lane's frame) inside a slot: row j, chunk (lane / 4) ^ (j & 7), word lane & 3.  Slots are
-  // 1024-byte aligned, so the swizzle is an XOR of (j & 7) << 4 into (slot + lane_off) -- one register instead of a table.
-  const uint32_t lane_off = (uint32_t)(((lane >> 2) << 4) | ((lane & 3) << 2));
-  // transposed view for the statistics: lane -> channel lane / 2, frames 16 * (lane & 1) .. + 15 (four 16-byte chunks k:
-  // chunk ((half * 4 + k) ^ (channel & 7)) = offset t_off ^ (k << 4))
-  const int sch = lane >> 1, shalf = lane & 1;
-  const uint32_t t_off = (uint32_t)(sch * 128 + ((((shalf << 2)) ^ (sch & 7)) << 4));
-  if (et < 128) bsm[et] = (a.bias && et < Cout_) ? a.bias[et] : 0.f;
-  asm volatile("bar.sync 5, %0;" ::"n"(NUM_EPI));
-  // request the residual values of the step `ahead` steps after (tile_, gi_) into ring position p (one commit group per step,
-  // also when there is nothing to copy, so that the group count identifies the step)
-  auto issue = [&](int tile_, int gi_, int ahead, int p) {
-    if (has_res) {
-      const int s_ = gi_ + ahead;
-      const int dt = s_ / ng;
-      const int gi = s_ - dt * ng;
-      tile_ += dt * (int)gridDim.x;
-      if (tile_ < ntiles) {
-        const int tq_ = tile_ % n_tq, b_ = tile_ / n_tq;
-        const int ncols_ = min(TN, Lq_ - tq_ * TN);
-        const int oidx_ = (tq_ * TN + tl) * ytst_ + ytoff_;
-        const float* r0 = a.res + (unsigned long long)(unsigned)b_ * (unsigned long long)a.res_bstride + (long long)(gi * 16) * res_len_ + (oidx_ >> rshift_);
-        const uint32_t dst = slot_base(p);
-        if (ncols_ - fr0 >= 32 && gi * 16 + 16 <= Cout_) {   // warp-uniform: full step
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(((dst + lane_off) ^ (uint32_t)((j & 7) << 4)) + 128u * j), "l"(r0) : "memory");
-            r0 += (unsigned)res_len_;
-          }
-        } else if (tl < ncols_) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (gi * 16 + j < Cout_)
-              asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(((dst + lane_off) ^ (uint32_t)((j & 7) << 4)) + 128u * j), "l"(r0 + (unsigned)j * (unsigned)res_len_) : "memory");
-          }
-        }
-      }
-      asm volatile("cp.async.commit_group;" ::: "memory");
-    }
-  };
-  for (int p = 0; p < D; ++p) issue(blockIdx.x, 0, p, p);
-  // HAS_ACC: the y values of the NEXT step (zeros where the frame or channel does not exist), one step ahead in registers
-  float yon[16];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) yon[j] = 0.f;
-  auto load_y = [&](int tile_, int gi_, int ahead) {
-    if (HAS_ACC) {
-      const int s_ = gi_ + ahead;
-      const int dt = s_ / ng;
-      const int gi = s_ - dt * ng;
-      tile_ += dt * (int)gridDim.x;
-      if (tile_ < ntiles) {
-        const int tq_ = tile_ % n_tq, b_ = tile_ / n_tq;
-        const bool tv_ = tl < min(TN, Lq_ - tq_ * TN);
-        const float* y0 = a.y + (unsigned long long)(unsigned)b_ * (unsigned long long)a.y_bstride + (long long)(gi * 16) * y_len_ + ((tq_ * TN + tl) * ytst_ + ytoff_);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          yon[j] = (tv_ && gi * 16 + j < Cout_) ? *y0 : 0.f;
-          y0 += (unsigned)y_len_;
-        }
-      }
-    }
-  };
-  load_y(blockIdx.x, 0, 0);
-  int it = 0, buf = 0, tph = 0, rp = 0;
-  for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-    const int tq = tile % n_tq, b = tile / n_tq;
-    const int ncols = min(TN, Lq_ - tq * TN);
-    const bool tv = tl < ncols;
-    const int nvalid = max(0, min(32, ncols - fr0));   // warp-uniform
-    float* yp = a.y + (unsigned long long)(unsigned)b * (unsigned long long)a.y_bstride + ((tq * TN + tl) * ytst_ + ytoff_);
-    float* sst = sstat + ((it & 1) * 8 + ewi) * NC * 3;
-    mbar_wait(BAR(T_TFULL + buf), tph);
-    tc_fence_after();
-    for (int gi = 0; gi < ng; ++gi) {
-      const int c0 = gi * 16;
-      float v[16];
-      tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * 2 * NC + m * NC + c0), v);
-      if (gi + 1 == ng) {   // last group: the accumulator buffer is free again
-        tc_fence_before();
-        mbar_arrive(BAR(T_TEMPTY + buf));
-      }
-      const int nch = min(16, Cout_ - c0);   // warp-uniform, may be <= 0 for padded channel groups
-      const bool full = (nch == 16) && (nvalid == 32) && plain;   // warp-uniform
-      const uint32_t slot = slot_base(rp);
-      float rv[16];
-      if (has_res) {
-        // this step's copies have landed when at most D-1 newer groups are pending
-        if (D == 3) asm volatile("cp.async.wait_group 2;" ::: "memory");
-        else asm volatile("cp.async.wait_group 1;" ::: "memory");
-        if (full) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) asm volatile("ld.shared.f32 %0, [%1];" : "=f"(rv[j]) : "r"(((slot + lane_off) ^ (uint32_t)((j & 7) << 4)) + 128u * j) : "memory");
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float r = 0.f;
-            if (tv && j < nch) asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(((slot + lane_off) ^ (uint32_t)((j & 7) << 4)) + 128u * j) : "memory");
-            rv[j] = r;
-          }
-        }
-      }
-      float* yp0 = yp + (long long)c0 * y_len_;
-      const float* bs0 = bsm + c0;
-      const unsigned ys = (unsigned)y_len_;
-      if (full) {
-        if (HAS_ACC) {
-          if (has_res) {
-            if (acc_ == 1) tct_rows_full<true, 1>(v, rv, yon, bs0, yp0, ys, acc_div_);
-            else tct_rows_full<true, 2>(v, rv, yon, bs0, yp0, ys, acc_div_);
-          } else {
-            if (acc_ == 1) tct_rows_full<false, 1>(v, rv, yon, bs0, yp0, ys, acc_div_);
-            else tct_rows_full<false, 2>(v, rv, yon, bs0, yp0, ys, acc_div_);
-          }
-        } else {
-          if (has_res) tct_rows_full<true, 0>(v, rv, yon, bs0, yp0, ys, acc_div_);
-          else tct_rows_full<false, 0>(v, rv, yon, bs0, yp0, ys, acc_div_);
-        }
-        load_y(tile, gi, 1);   // (HAS_ACC) y of the next step: in flight during the statistics and the next step's TMEM load
-        if (has_stats) {
-          // values back into the slot (each lane overwrites the words its residuals came from), read transposed
-#pragma unroll
-          for (int j = 0; j < 16; ++j) asm volatile("st.shared.f32 [%0], %1;" ::"r"(((slot + lane_off) ^ (uint32_t)((j & 7) << 4)) + 128u * j), "f"(v[j]) : "memory");
-          __syncwarp();
-          float x[16];
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x[4 * k]), "=f"(x[4 * k + 1]), "=f"(x[4 * k + 2]), "=f"(x[4 * k + 3]) : "r"((slot + t_off) ^ (uint32_t)(k << 4)) : "memory");
-          float sum = 0.f;
-#pragma unroll
-          for (int k = 0; k < 16; ++k) sum += x[k];
-          const float mh = sum * (1.0f / 16.0f);
-          float qh = 0.f;
-#pragma unroll
-          for (int k = 0; k < 16; ++k) { const float d = x[k] - mh; qh = fmaf(d, d, qh); }
-          // the two halves of a channel sit in neighbouring lanes: Chan merge of two 16-sample records
-          const float mo = __shfl_xor_sync(0xffffffffu, mh, 1), qo = __shfl_xor_sync(0xffffffffu, qh, 1);
-          const float dl = mo - mh;
-          if (shalf == 0) {
-            float* sp = sst + (c0 + sch) * 3;
-            sp[0] = 32.0f; sp[1] = mh + 0.5f * dl; sp[2] = qh + qo + dl * dl * 8.0f;
-          }
-          __syncwarp();   // every lane has read the slot: it may be refilled
-        }
-      } else if (nch > 0 && nvalid > 0) {
-        if (has_res) {
-          if (acc_ == 0) tct_rows<true, 0>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-          else if (acc_ == 1) tct_rows<true, 1>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-          else tct_rows<true, 2>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-        } else {
-          if (acc_ == 0) tct_rows<false, 0>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-          else if (acc_ == 1) tct_rows<false, 1>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-          else tct_rows<false, 2>(v, rv, bs0, yp0, ys, nch, tv, out_div_, acc_div_, out_act_);
-        }
-        load_y(tile, gi, 1);
-        if (has_stats) {
-          // partial step (tail tile / channel tail / output activation): transposing shuffle tree over the valid frames,
-          // deviations from a pilot sample per channel = the value of the warp's first frame (valid when nvalid > 0)
-          if (lane == 0) {
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4)
-              *reinterpret_cast<float4*>(&pil[4 * k4]) = make_float4(v[4 * k4], v[4 * k4 + 1], v[4 * k4 + 2], v[4 * k4 + 3]);
-          }
-          __syncwarp();
-#pragma unroll
-          for (int k4 = 0; k4 < 4; ++k4) {
-            const float4 p4 = *reinterpret_cast<const float4*>(&pil[4 * k4]);
-            v[4 * k4] = tv ? v[4 * k4] - p4.x : 0.f;
-            v[4 * k4 + 1] = tv ? v[4 * k4 + 1] - p4.y : 0.f;
-            v[4 * k4 + 2] = tv ? v[4 * k4 + 2] - p4.z : 0.f;
-            v[4 * k4 + 3] = tv ? v[4 * k4 + 3] - p4.w : 0.f;
-          }
-          {  // lanes L and L^16 hold the same 16 channels: the lower lane continues with the sums, the upper one with the squares
-            const bool up = (lane & 16) != 0;
-#pragma unroll
-            for (int i = 0; i < 16; ++i) {
-              const float o = __shfl_xor_sync(0xffffffffu, v[i], 16);
-              v[i] = up ? fmaf(v[i], v[i], o * o) : v[i] + o;
-            }
-          }
-          xreduce_step<8>(v, lane);
-          xreduce_step<4>(v, lane);
-          xreduce_step<2>(v, lane);
-          xreduce_step<1>(v, lane);
-          // lane L < 16: S1 (sum of deviations from the pilot) of channel c0 + L; lane 16 + L: S2 (sum of their squares)
-          const float s2 = __shfl_down_sync(0xffffffffu, v[0], 16);
-          const float nn = (float)nvalid;
-          const float pl = pil[lane & 15];
-          if (lane < nch) {
-            float* sp = sst + (c0 + lane) * 3;
-            sp[0] = nn; sp[1] = pl + v[0] / nn; sp[2] = fmaxf(0.f, s2 - v[0] * v[0] / nn);
-          }
-          __syncwarp();
-        }
-      } else {
-        load_y(tile, gi, 1);
-      }
-      issue(tile, gi, D, rp);   // the slot is free again: the step D steps ahead
-      if (++rp == D) rp = 0;
-    }
-    if (has_stats) {
-      if (nvalid == 0) {   // this warp's frames are beyond the row: empty records for every channel
-        for (int c = lane; c < Cout_; c += 32) { sst[c * 3] = 0.f; sst[c * 3 + 1] = 0.f; sst[c * 3 + 2] = 0.f; }
-      }
-      // the four warps of an M block merge their records in fixed order: one partial per (tile, M block, channel)
-      asm volatile("bar.sync %0, 128;" ::"r"(3 + m) : "memory");
-      const int co = et & 127;
-      if (co < Cout_) {
-        float n = 0.f, mean = 0.f, m2 = 0.f;
-#pragma unroll
-        for (int qq = 0; qq < 4; ++qq) {
-          const float* sp = sstat + (((it & 1) * 8 + m * 4 + qq) * NC + co) * 3;
-          const float nb = sp[0], mb = sp[1], qb = sp[2];
-          if (nb > 0.f) {
-            const float nn = n + nb, dl = mb - mean;
-            mean += dl * (nb / nn);
-            m2 += qb + dl * dl * (n * nb / nn);
-            n = nn;
-          }
-        }
-        float* gp = a.stats + (((long long)b * Cout_ + co) * a.stats_nparts + a.stats_part_offset + 2 * tq + m) * 3;
-        gp[0] = n; gp[1] = mean; gp[2] = m2;
-      }
-    }
-    if (++buf == NBUF) { buf = 0; tph ^= 1; }
-  }
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-}
-
+template <int NH>
 __global__ void __launch_bounds__(THREADS, 1)
-conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int ncb, const int RW, const int ntiles, const int n_tq,
-                  const int NC) {
+conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int ncb, const int RW, const int ntiles, const int n_tq) {
   constexpr int MODE = MODE_FAST;
+  constexpr int NC = 2 * NH;
+  constexpr int NJ = NH / 8;
   const int RWP = RW + 2;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SM_BAR;
   auto BAR = [&](int i) { return bar0 + 8u * i; };
-  // accumulator ring: NBUF = 512 / (2 NC) buffers of two M blocks (2 for NC = 128 ... 8 for NC <= 32): the MMAs run up to
-  // NBUF tiles ahead of the epilogue, whose steps wait for residual rows from HBM
-  const int NBUF = min(T_MAXBUF, 512 / (2 * NC));
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 8 * 32);
 
   if (tid == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 1); }
+    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
     for (int i = 0; i < 2; ++i) {
       mbar_init(BAR(B_AFULL + i), NUM_STAGERS);
-      mbar_init(BAR(B_AEMPTY + i), 1);
-    }
-    for (int i = 0; i < T_MAXBUF; ++i) {
-      mbar_init(BAR(T_TFULL + i), 1);
-      mbar_init(BAR(T_TEMPTY + i), NUM_EPI);
+      mbar_init(BAR(B_AEMPTY + i), 2);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int K = a.K;
   const int wstep = 64 * NC;                      // bytes of one (16 channels, tap) step: 2 planes x 2 chunks x NC rows x 16 B
   const int tps = T_WSTAGE / wstep;               // taps per weight stage: 1 (NC = 128, 96) .. 8 (NC = 16)
 
-  if (warp == 0) {
-    // ================================================================ MMA issuer (converged warp, one elected lane)
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(NC >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);   // D = f32, M = 128, N = NC
-    const uint32_t elected = elect_one();
-    const uint64_t dx_d = make_desc(sbase + SM_ACT, (uint32_t)RWP * 16, 128), dw_d = make_desc(sbase + SM_W, (uint32_t)NC * 16, 128);
-    const uint32_t dx_lo0 = (uint32_t)dx_d, dx_hi = (uint32_t)(dx_d >> 32), dw_lo0 = (uint32_t)dw_d, dw_hi = (uint32_t)(dw_d >> 32);
-    const uint32_t dil_ = (uint32_t)a.dil, wplane16 = (uint32_t)(2 * NC), wstep16 = (uint32_t)(4 * NC);
-    int ws = 0, wph = 0, as = 0, aph = 0, buf = 0, tph = 0;
+  if (warp < NUM_CONS / 32) {
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+    const bool leader = (tid & 127) == 0;
+    const uint32_t lbo_x = (uint32_t)RWP * 16, lbo_w = (uint32_t)NC * 16;
+    const uint32_t dil16 = (uint32_t)a.dil * 16u;
+    float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * 64;   // [4 warps][64 channels]
+    int ws = 0, wph = 0, as = 0, aph = 0;
+    Pending pend{-1, -1};
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      mbar_wait(BAR(T_TEMPTY + buf), tph ^ 1);
-      tc_fence_after();
-      const uint32_t d0 = tmem_base + (uint32_t)(buf * 2 * NC);   // M block 0; M block 1 at + NC columns
+      const int tq = tile % n_tq, b = tile / n_tq;
+      float d[NH / 2], e[NH / 2];   // fp16 main products / e4m3 correction products (e4m3 wgmma accumulates at reduced precision)
+#pragma unroll
+      for (int i = 0; i < NH / 2; ++i) { d[i] = 0.f; e[i] = 0.f; }
       uint32_t acc = 0;
       for (int cb = 0; cb < ncb; ++cb) {
         mbar_wait(BAR(B_AFULL + as), aph);
-        tc_fence_after();
-        uint32_t x_lo = dx_lo0 + (uint32_t)as * (ACT_BUF_BYTES >> 4);
+        uint32_t x_addr = sbase + SM_ACT + as * ACT_BUF_BYTES;
         for (int tap0 = 0; tap0 < K; tap0 += tps) {
           mbar_wait(BAR(B_WFULL + ws), wph);
-          tc_fence_after();
+          wg_fence();
           const int nt = min(tps, K - tap0);
-          if (elected) {
-            uint32_t w_lo = dw_lo0 + (uint32_t)ws * (T_WSTAGE >> 4);
-            for (int t = 0; t < nt; ++t) {
-#pragma unroll
-              for (int m = 0; m < 2; ++m) {
-                tc_mma_w(d0 + (uint32_t)(m * NC), x_lo + 128u * m, dx_hi, w_lo, dw_hi, idesc, acc);
-                tc_mma_f8_w(d0 + (uint32_t)(m * NC), x_lo + 128u * m + (ACT_PLANE_BYTES >> 4), dx_hi, w_lo + wplane16, dw_hi, idesc, 1u);
-              }
-              acc = 1;
-              w_lo += wstep16;
-              x_lo += dil_;
-            }
-            tc_commit(BAR(B_WEMPTY + ws));
-          } else {
+          uint32_t w_addr = sbase + SM_W + ws * T_WSTAGE + wg * NH * 16;
+          for (int t = 0; t < nt; ++t) {
+            tct_mma<NH>(d, e, make_desc(x_addr, lbo_x, 128), make_desc(w_addr, lbo_w, 128), make_desc(x_addr + ACT_PLANE_BYTES, lbo_x, 128),
+                        make_desc(w_addr + 2 * NC * 16, lbo_w, 128), acc);
             acc = 1;
-            x_lo += dil_ * (uint32_t)nt;
+            w_addr += wstep;
+            x_addr += dil16;
           }
+          wg_commit();
+          wg_wait<1>();
+          release(bar0, pend, leader);
+          pend.ws = ws;
+          pend.as = (tap0 + tps >= K) ? as : -1;
           if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
         }
-        if (elected) tc_commit(BAR(B_AEMPTY + as));
         if (++as == 2) { as = 0; aph ^= 1; }
       }
-      if (elected) tc_commit(BAR(T_TFULL + buf));
-      if (++buf == NBUF) { buf = 0; tph ^= 1; }
+      wg_wait<0>();
+      wg_fence_regs(d);
+      wg_fence_regs(e);
+#pragma unroll
+      for (int i = 0; i < NH / 2; ++i) d[i] += e[i];
+      release(bar0, pend, leader);
+      pend.ws = -1;
+
+      // ---- epilogue: row = frame, column = output channel
+      const int t0 = tq * TN;
+      const int ncols = min(TN, a.Lq - t0);
+      float* yb = a.y + (long long)b * a.y_bstride;
+      const float* rbase = a.res ? a.res + (long long)b * a.res_bstride : nullptr;
+      float s[NJ * 2], n[NJ * 2];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int co = wg * NH + 8 * j + 2 * t4 + c;
+          const bool cok = co < a.Cout;
+          const float bias = (a.bias && cok) ? a.bias[co] : 0.f;
+          float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+          const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
+          float ss = 0.f, nn = 0.f;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const int fr = w * 16 + g + 8 * i;
+            const int r = 4 * j + 2 * i + c;
+            float val = 0.f;
+            if (cok && fr < ncols) {
+              val = epi_value(a, d[r] * D_UNSCALE, bias, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset);
+              ss += val;
+              nn += 1.f;
+            }
+            d[r] = val;
+          }
+          s[2 * j + c] = ss;
+          n[2 * j + c] = nn;
+        }
+      }
+      if (a.stats) {
+        const uint32_t bar_id = 3 + wg;
+        // pass 1: sums over the 16 frames of the warp (lanes with equal t4), then over the warpgroup's four warps
+#pragma unroll
+        for (int k = 0; k < 2 * NJ; ++k) {
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
+            n[k] += __shfl_xor_sync(0xffffffffu, n[k], o);
+          }
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the previous tile's readers are done
+        if (g == 0) {
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) red[w * 64 + 8 * j + 2 * t4 + c] = s[2 * j + c];
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        float mean[2 * NJ], cnt[2 * NJ];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int ch = 8 * j + 2 * t4 + c;
+            const float tot = red[ch] + red[64 + ch] + red[128 + ch] + red[192 + ch];
+            // count of the tile = valid frames (the same for every existing channel)
+            cnt[2 * j + c] = (float)max(0, ncols);
+            mean[2 * j + c] = ncols > 0 ? tot / (float)ncols : 0.f;
+          }
+        // pass 2: M2 about the tile mean
+        float q[2 * NJ];
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            float m2 = 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int fr = w * 16 + g + 8 * i;
+              const float dv = d[4 * j + 2 * i + c] - mean[2 * j + c];
+              if (fr < ncols) m2 = fmaf(dv, dv, m2);
+            }
+#pragma unroll
+            for (int o = 4; o < 32; o <<= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
+            q[2 * j + c] = m2;
+          }
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        if (g == 0) {
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) red[w * 64 + 8 * j + 2 * t4 + c] = q[2 * j + c];
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
+        if (w == 0 && g == 0) {
+#pragma unroll
+          for (int j = 0; j < NJ; ++j)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int ch = 8 * j + 2 * t4 + c, co = wg * NH + ch;
+              if (co < a.Cout) {
+                float* gp = a.stats + (((long long)b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + tq) * 3;
+                gp[0] = cnt[2 * j + c];
+                gp[1] = mean[2 * j + c];
+                gp[2] = red[ch] + red[64 + ch] + red[128 + ch] + red[192 + ch];
+              }
+            }
+        }
+      }
     }
-  } else if (warp == 1) {
+  } else if (warp == NUM_CONS / 32) {
     // ================================================================ weight producer (1-D TMA bulk copies)
     if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, wstep, tps, T_WSTAGE, ntiles, n_tq, 1);
-  } else if (warp < 2 + NUM_STAGERS / 32) {
-    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, 1, tid, warp, lane);
   } else {
-    if (a.accum_mode != 0) tct_epilogue_role<true>(a, smem, sbase, bar0, tmem_base, ntiles, n_tq, NC, NBUF, tid, warp, lane);
-    else tct_epilogue_role<false>(a, smem, sbase, bar0, tmem_base, ntiles, n_tq, NC, NBUF, tid, warp, lane);
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512));
+    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, 1, tid, warp, lane);
   }
 }
 
@@ -1316,14 +780,11 @@ __device__ __forceinline__ void weight_stage_store(uint8_t* blk, int byte_in_sta
   }
 }
 
-// Row `col` of output-channel block `cob` -> output channel (or -1): channel-major layout spreads the channels over the four
-// TMEM lane quarters (rows_per_quarter), the time-major layout (rows = NC, one block) is the identity.
+// Row `col` of output-channel block `cob` -> output channel (or -1): rows are the channels of the block in order (the
+// time-major layout has one block of NC rows).
 __device__ __forceinline__ int weight_row_channel(int Cout, int cob, int col, bool tmajor) {
-  if (tmajor) return col < Cout ? col : -1;
-  const int rq = rows_per_quarter(Cout, cob);
-  const int qq = col >> 5, rr = col & 31;
-  const int co = cob * TM + qq * rq + rr;
-  return (rr < rq && co < Cout) ? co : -1;
+  const int co = tmajor ? col : cob * TM + col;
+  return co < Cout ? co : -1;
 }
 
 // fp32 [Cout,Cin,K] -> step blocks [n_cob][ncb][K] x (64 * rows) bytes (the taps of one 16-channel block are contiguous)
@@ -1468,11 +929,22 @@ static int launch_tc(const st2_conv_args& a, const void* wtc, int mode, int max_
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_ACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
-    cudaFuncSetAttribute(conv1d_tct_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    cudaFuncSetAttribute(conv1d_tct_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    cudaFuncSetAttribute(conv1d_tct_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    cudaFuncSetAttribute(conv1d_tct_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    cudaFuncSetAttribute(conv1d_tct_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
+    cudaFuncSetAttribute(conv1d_tct_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
   }
   int grid = ntiles < num_sms[dev] ? ntiles : num_sms[dev];
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  if (tmajor) conv1d_tct_kernel<<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq, tmajor_nc(a.Cout));
+  if (tmajor) {
+    const int nh = tmajor_nc(a.Cout) / 2;
+    if (nh == 8) conv1d_tct_kernel<8><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq);
+    else if (nh == 16) conv1d_tct_kernel<16><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq);
+    else if (nh == 32) conv1d_tct_kernel<32><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq);
+    else if (nh == 48) conv1d_tct_kernel<48><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq);
+    else conv1d_tct_kernel<64><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq);
+  }
   else if (mode == MODE_FAST) conv1d_tc_kernel<MODE_FAST><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq, n_cob);
   else if (mode == MODE_ACC) conv1d_tc_kernel<MODE_ACC><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq, n_cob);
   else conv1d_tc_kernel<MODE_X3><<<grid, THREADS, SM_TOTAL, st>>>(a, (const uint4*)wtc, ncb, rw, ntiles, n_tq, n_cob);
@@ -1522,7 +994,7 @@ int st2_conv1d_tc(const st2_conv_args* a, const void* wtc, int mode, int max_cta
   ST2_REQUIRE(a->pre_act != ST2_ACT_SNAKE || a->pre_alpha, "st2_conv1d_tc", "snake prologue needs alpha");
   ST2_REQUIRE(!(mode & tc::TMAJOR) || a->dup_q0_to < 0, "st2_conv1d_tc", "time-major kernel: no reflection duplicate");
   const int n_tq = cdiv(a->Lq, tc::TN);
-  ST2_REQUIRE(!a->stats || a->stats_nparts >= a->stats_part_offset + 2 * n_tq, "st2_conv1d_tc", "stats buffer too small (2 partials per 256-column tile)");
+  ST2_REQUIRE(!a->stats || a->stats_nparts >= a->stats_part_offset + n_tq, "st2_conv1d_tc", "stats buffer too small (one partial per 64-column tile)");
   tc::launch_tc(*a, wtc, mode, max_ctas, (cudaStream_t)stream);
   ST2_CHECK_LAUNCH("st2_conv1d_tc");
   return 0;
@@ -1563,7 +1035,7 @@ int st2_conv_transpose1d_tc(const st2_conv_args* a0, const void* wtc, int mode, 
   ST2_REQUIRE(K > 0 && S > 0 && P >= 0, "st2_conv_transpose1d_tc", "bad shape");
   const int J = (K + S - 1) / S;
   ST2_REQUIRE(st2_conv_tc_supported(a0->Cin, a0->Cout, J, 1, 1), "st2_conv_transpose1d_tc", "unsupported shape");
-  const int parts = 2 * cdiv(a0->Lin, tc::TN);
+  const int parts = cdiv(a0->Lin, tc::TN);
   ST2_REQUIRE(!a0->stats || a0->stats_nparts >= S * parts, "st2_conv_transpose1d_tc", "stats buffer too small");
   const long long phase_bytes = st2_conv_tc_weight_bytes(a0->Cout, a0->Cin, J);
   for (int r = 0; r < S; ++r) {

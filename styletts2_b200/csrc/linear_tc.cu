@@ -1,4 +1,4 @@
-// Tensor-core (tcgen05 / TMEM) GEMM for the row-layout Linears of the style denoiser -- sm_100a.
+// Tensor-core (wgmma) GEMM for the row-layout Linears of the style denoiser -- sm_90a.
 //
 //   C[m, n] = act( sum_k A[m,k] * W[n,k] + bias[n] ) + R[m,n]         A,C,R row-major, W = torch Linear weight [Nf,K]
 //
@@ -6,19 +6,19 @@
 // arithmetic must stay at fp32 accuracy (DESIGN.md section 2).  Every operand is split into TWO fp16 planes,
 // x = h + l * 2^-11 with h = fp16(x) and l = fp16((x - h) * 2^11): 22 significand bits, and the 2^11 pre-scaling keeps
 // the low plane out of fp16's subnormal range for every |x| >= 2^-14.  A product needs the three MMAs h*h, h*l, l*h
-// (l*l is 2^-22 relative); h*h accumulates in one TMEM accumulator and the two scaled correction products in a
-// second one that the epilogue folds in with an exact * 2^-11 (the first version used three bf16 planes and six
-// MMAs per product for the same accuracy: measured error equal, denoiser time halved).
+// (l*l is 2^-22 relative); h*h accumulates in one register accumulator and the two scaled correction products in a
+// second one that the epilogue folds in with an exact * 2^-11 (the tensor core truncates when it adds into an
+// accumulator, so keeping the small terms out of the big running sum keeps the error at the fp32-SIMT level).
 // Range: |x| must stay below fp16's 65504 (activations and weights of this model are O(1..10)); larger values
 // produce inf/NaN loudly rather than a silently wrong result.
 //
-// Mapping (same machinery as conv_tc.cu): D[128 out-features (UMMA M) x 128 tokens (UMMA N)] in TMEM (2 x 128 columns,
-// double buffered).  A operand = weight block [128 n x 16 k], B operand = activation block [128 tokens x 16 k], both
-// K-major no-swizzle "interleave" layout (16-byte rows of 8 fp16).  Weights are pre-split and pre-arranged so that
-// one K-block stage (32 features x 2 planes) is one contiguous 16 KB 1-D TMA bulk copy.  Activations are staged by
-// 8 warps (two threads per token row: 64 contiguous bytes each, software-pipelined one block ahead).  The epilogue
-// needs no transpose: TMEM lane = out-feature, so for each token column the 32 lanes write 32 consecutive floats.
-// Warp roles: warp 0 MMA issue, warp 1 TMA producer, warps 2-9 stagers, warps 10-13 epilogue; persistent CTAs.
+// Mapping: a tile is 128 out-features x 64 tokens.  A operand = weight block [64 n x 16 k] per warpgroup, B operand =
+// activation block [64 tokens x 16 k], both K-major no-swizzle "interleave" layout (16-byte rows of 8 fp16).  Weights are
+// pre-split and pre-arranged so that one K-block stage (32 features x 2 planes) is one contiguous 16 KB 1-D TMA bulk copy.
+// Activations are staged by 8 warps (four threads per token row, 32 contiguous bytes each, software-pipelined one block
+// ahead) or arrive pre-split as one bulk copy per stage.
+// Warp roles: warps 0-7 = two consumer warpgroups (wgmma over out-features 0-63 / 64-127, accumulators in registers, then
+// the epilogue), warp 8 = TMA producer, warps 9-16 = stagers; persistent CTAs.
 #include <cuda_fp16.h>
 
 #include "common.cuh"
@@ -29,8 +29,8 @@ extern long long g_launches;
 
 namespace ltc {
 
-constexpr int TMF = 128;   // out features per tile (UMMA M)
-constexpr int TNT = 128;   // tokens per tile (UMMA N)
+constexpr int TMF = 128;   // out features per tile (two warpgroups of M = 64)
+constexpr int TNT = 64;    // tokens per tile (wgmma N)
 constexpr int KB = 32;     // K block (4 chunks of 8)
 constexpr int NPL = 2;     // fp16 planes per operand (high, low * 2^11)
 constexpr float LO_SCALE = 2048.0f, LO_UNSCALE = 1.0f / 2048.0f;
@@ -38,21 +38,20 @@ constexpr int W_STAGES = 6;
 constexpr int W_PLANE_BYTES = 4 * TMF * 16;          // 8 KB
 constexpr int W_STAGE_BYTES = NPL * W_PLANE_BYTES;   // 16 KB
 constexpr int RWP = TNT + 2;                         // chunk pitch in rows (== 2 mod 8: conflict-free 128-bit stores)
-constexpr int A_PLANE_BYTES = 4 * RWP * 16;          // 8320 B
-constexpr int A_BUF_BYTES = NPL * A_PLANE_BYTES;     // 16640 B
+constexpr int A_PLANE_BYTES = 4 * RWP * 16;          // 4224 B
+constexpr int A_BUF_BYTES = NPL * A_PLANE_BYTES;
 constexpr int A_BUFS = 4;
-constexpr int PRE_PLANE_BYTES = 4 * TNT * 16;         // pre-split stage: no row padding, 8 KB per plane, 16 KB per stage
+constexpr int PRE_PLANE_BYTES = 4 * TNT * 16;         // pre-split stage: no row padding, 4 KB per plane, 8 KB per stage
 constexpr int PRE_STAGE_BYTES = NPL * PRE_PLANE_BYTES;
+constexpr int NUM_CONS = 256;                        // two consumer warpgroups
 constexpr int NUM_STAGERS = 256;
-constexpr int NUM_EPI = 128;
-constexpr int THREADS = 64 + NUM_STAGERS + NUM_EPI;  // 448 (14 warps -> 16-warp allocation, 128 regs)
-constexpr int TMEM_COLS = 512;  // 2 buffers x (hi accumulator 128 cols + lo accumulator 128 cols)
+constexpr int THREADS = NUM_CONS + 32 + NUM_STAGERS;  // 544
 
 constexpr int SM_W = 0;
 constexpr int SM_A = SM_W + W_STAGES * W_STAGE_BYTES;
 constexpr int SM_BAR = SM_A + A_BUFS * A_BUF_BYTES;
 constexpr int SM_TOTAL = SM_BAR + 256;
-constexpr int B_WFULL = 0, B_WEMPTY = 6, B_AFULL = 12, B_AEMPTY = 16, B_TFULL = 20, B_TEMPTY = 22, B_COUNT = 24;
+constexpr int B_WFULL = 0, B_WEMPTY = 6, B_AFULL = 12, B_AEMPTY = 16, B_COUNT = 20;
 
 using namespace st2::ptx;
 
@@ -65,13 +64,6 @@ __device__ __forceinline__ void range_note(float amax) {
   if (!(amax < FP16_MAX)) atomicExch(&g_range_flag, 1);   // also catches NaN
 }
 
-__device__ __forceinline__ uint32_t make_idesc() {
-  uint32_t d = 0;
-  d |= 1u << 4;                      // D = F32;  A = B = F16 (format code 0 in bits 7-9 / 10-12)
-  d |= (uint32_t)(TNT >> 3) << 17;   // N
-  d |= (uint32_t)(TMF >> 4) << 24;   // M
-  return d;
-}
 // x0,x1 -> two packed fp16 pairs: p0 = fp16(x), p1 = fp16((x - p0) * 2^11)   (x = p0 + p1 * 2^-11 to ~2^-22 |x|)
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& p0, uint32_t& p1) {
   const __half2 h = __floats2half2_rn(x0, x1);
@@ -97,72 +89,78 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SM_BAR;
   auto BAR = [&](int i) { return bar0 + 8u * i; };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + SM_BAR + 8 * B_COUNT);
   if (tid == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 1); }
-    for (int i = 0; i < A_BUFS; ++i) { mbar_init(BAR(B_AFULL + i), a.planes ? 1 : NUM_STAGERS); mbar_init(BAR(B_AEMPTY + i), 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(BAR(B_TFULL + i), 1); mbar_init(BAR(B_TEMPTY + i), NUM_EPI); }
+    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
+    for (int i = 0; i < A_BUFS; ++i) { mbar_init(BAR(B_AFULL + i), a.planes ? 1 : NUM_STAGERS); mbar_init(BAR(B_AEMPTY + i), 2); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    // ================================================================ MMA issuer
-    // the whole warp stays converged on the barrier waits, ONE elected lane issues; descriptors as (low, high) words so
-    // that a K step only bumps the low word (see conv_tc.cu: a lone lane walking a generic loop costs as many cycles in
-    // dependent instructions as the MMAs of a stage take on the tensor pipe)
-    {
-      const uint32_t idesc = make_idesc();
-      const uint32_t elected = elect_one();
-      const uint32_t lbo_a = TMF * 16, lbo_b = (a.planes ? TNT : RWP) * 16;
-      const uint32_t a_plane16 = (a.planes ? (uint32_t)PRE_PLANE_BYTES : (uint32_t)A_PLANE_BYTES) >> 4;
-      const uint64_t da_d = make_desc(sbase + SM_W, lbo_a, 128), db_d = make_desc(sbase + SM_A, lbo_b, 128);
-      const uint32_t da_lo0 = (uint32_t)da_d, da_hi = (uint32_t)(da_d >> 32), db_lo0 = (uint32_t)db_d, db_hi = (uint32_t)(db_d >> 32);
-      int ws = 0, wph = 0, as = 0, aph = 0, it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int buf = it & 1;
-        mbar_wait(BAR(B_TEMPTY + buf), ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        // Two accumulators per tile: D_hi takes only the leading products h*h, D_lo the two correction products (kept
-        // 2^11 times larger than their true weight).  The tensor core truncates when it adds into an accumulator, so
-        // keeping the small terms out of the big running sum also cuts the accumulation error (measured with the
-        // bf16 version: 4.4e-6 -> fp32-SIMT level at K=1024).
-        const uint32_t d_hi = tmem_base + (uint32_t)buf * (2 * TNT);
-        const uint32_t d_lo = d_hi + TNT;
-        uint32_t acc = 0;
-        for (int cb = 0; cb < ncb; ++cb) {
-          mbar_wait(BAR(B_AFULL + as), aph);
-          mbar_wait(BAR(B_WFULL + ws), wph);
-          tc_fence_after();
-          if (elected) {
-            const uint32_t wa = da_lo0 + (uint32_t)ws * (W_STAGE_BYTES >> 4), ab = db_lo0 + (uint32_t)as * (A_BUF_BYTES >> 4);
+  if (warp < NUM_CONS / 32) {
+    // ================================================================ consumers: wgmma + epilogue
+    const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
+    const bool leader = (tid & 127) == 0;
+    const uint32_t lbo_a = TMF * 16, lbo_b = (a.planes ? TNT : RWP) * 16;
+    const uint32_t a_plane = a.planes ? (uint32_t)PRE_PLANE_BYTES : (uint32_t)A_PLANE_BYTES;
+    const int M_ = a.M, Nf_ = a.Nf, act_ = a.act;
+    int ws = 0, wph = 0, as = 0, aph = 0;
+    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+      const int cob = tile / n_tq, tq = tile % n_tq;
+      float dh[32], dl[32];
 #pragma unroll
-            for (int k16 = 0; k16 < 2; ++k16) {
-              const uint32_t a0 = wa + (uint32_t)(2 * k16) * (lbo_a >> 4), a1 = a0 + (W_PLANE_BYTES >> 4);
-              const uint32_t b0 = ab + (uint32_t)(2 * k16) * (lbo_b >> 4), b1 = b0 + a_plane16;
-              tc_mma_w(d_hi, a0, da_hi, b0, db_hi, idesc, acc);
-              tc_mma_w(d_lo, a0, da_hi, b1, db_hi, idesc, acc);
-              tc_mma_w(d_lo, a1, da_hi, b0, db_hi, idesc, 1u);
-              acc = 1;
-            }
-            tc_commit(BAR(B_WEMPTY + ws));
-            tc_commit(BAR(B_AEMPTY + as));
-          }
-          acc = 1;
-          if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-          if (++as == A_BUFS) { as = 0; aph ^= 1; }
+      for (int i = 0; i < 32; ++i) { dh[i] = 0.f; dl[i] = 0.f; }
+      int pws = -1, pas = -1;
+      for (int cb = 0; cb < ncb; ++cb) {
+        mbar_wait(BAR(B_AFULL + as), aph);
+        mbar_wait(BAR(B_WFULL + ws), wph);
+        wg_fence();
+        const uint32_t wa = sbase + SM_W + ws * W_STAGE_BYTES + wg * 64 * 16, ab = sbase + SM_A + as * A_BUF_BYTES;
+#pragma unroll
+        for (int k16 = 0; k16 < 2; ++k16) {
+          const uint64_t a0 = make_desc(wa + 2 * k16 * lbo_a, lbo_a, 128), a1 = make_desc(wa + 2 * k16 * lbo_a + W_PLANE_BYTES, lbo_a, 128);
+          const uint64_t b0 = make_desc(ab + 2 * k16 * lbo_b, lbo_b, 128), b1 = make_desc(ab + 2 * k16 * lbo_b + a_plane, lbo_b, 128);
+          const uint32_t acc = (cb | k16) ? 1u : 0u;
+          wgmma_f16_n64(dh, a0, b0, acc);
+          wgmma_f16_n64(dl, a0, b1, acc);
+          wgmma_f16_n64(dl, a1, b0, 1u);
         }
-        if (elected) tc_commit(BAR(B_TFULL + buf));
+        wg_commit();
+        // keep one stage of MMAs in flight: the previous stage's operands are free once at most one group is pending
+        wg_wait<1>();
+        if (pws >= 0 && leader) { mbar_arrive(BAR(B_WEMPTY + pws)); mbar_arrive(BAR(B_AEMPTY + pas)); }
+        pws = ws; pas = as;
+        if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
+        if (++as == A_BUFS) { as = 0; aph ^= 1; }
+      }
+      wg_wait<0>();
+      wg_fence_regs(dh);
+      wg_fence_regs(dl);
+      if (leader) { mbar_arrive(BAR(B_WEMPTY + pws)); mbar_arrive(BAR(B_AEMPTY + pas)); }
+      // epilogue from the fragments: feature n = row, token m = column
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int n = cob * TMF + wg * 64 + w * 16 + g + 8 * i;
+        const bool nok = n < Nf_;
+        const float bias = (a.bias && nok) ? a.bias[n] : 0.f;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int m = tq * TNT + 8 * j + 2 * t4 + c;
+            const int r = 4 * j + 2 * i + c;
+            float val = fmaf(dl[r], LO_UNSCALE, dh[r]) + bias;
+            if (act_ == ST2_ACT_GELU) val = gelu_erf(val);
+            else if (act_ == ST2_ACT_TANH) val = tanhf(val);
+            else if (act_ == ST2_ACT_GELU_TANH) val = gelu_tanh(val);
+            if (nok && m < M_) {
+              if (a.R) val += a.R[(long long)m * a.ldr + n];
+              a.C[(long long)m * a.ldc + n] = val;
+            }
+          }
+        }
       }
     }
-  } else if (warp == 1) {
+  } else if (warp == NUM_CONS / 32) {
     // ================================================================ weight producer
     if (lane == 0) {
       int ws = 0, wph = 0;
@@ -177,16 +175,16 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
         }
       }
     }
-  } else if (warp < 2 + NUM_STAGERS / 32) {
+  } else {
     // ================================================================ activation stagers
-    // thread -> token row (st >> 1) and half of the 32-feature block (st & 1): 16 contiguous floats = 4 x 128-bit loads;
-    // the loads of block cb+1 are issued before block cb is converted (software pipeline).
-    const int st = tid - 64;
-    const int row = st >> 1, hf = st & 1;
+    // thread -> token row (st >> 2) and 8-feature chunk (st & 3) of the 32-feature block: 8 contiguous floats = 2 x 128-bit
+    // loads; the loads of block cb+1 are issued before block cb is converted (software pipeline).
+    const int st = tid - (NUM_CONS + 32);
+    const int row = st >> 2, kc = st & 3;
     const int K_ = a.K, M_ = a.M;
     int as = 0, aph = 0;
     if (a.planes) {
-      // pre-split activations: every (token block, K block) stage is one contiguous 16 KB image of the operand buffer
+      // pre-split activations: every (token block, K block) stage is one contiguous image of the operand buffer
       if (st == 0) {
         for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
           const int tq = tile % n_tq;
@@ -204,13 +202,13 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
       const int tq = tile % n_tq;
       const int m = tq * TNT + row;
       const bool mok = m < M_;
-      const float* ar = a.A + (long long)(mok ? m : 0) * a.lda + hf * 16;
+      const float* ar = a.A + (long long)(mok ? m : 0) * a.lda + kc * 8;
       const bool vec_ok = ((a.lda & 3) == 0) && ((reinterpret_cast<size_t>(a.A) & 15) == 0);
-      float4 cur[4], nxt[4];
-      auto load_blk = [&](int cb, float4 (&dst)[4]) {
-        const int k0 = cb * KB + hf * 16;
+      float4 cur[2], nxt[2];
+      auto load_blk = [&](int cb, float4 (&dst)[2]) {
+        const int k0 = cb * KB + kc * 8;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) {
+        for (int q = 0; q < 2; ++q) {
           const int k = k0 + 4 * q;
           float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
           if (mok) {
@@ -230,81 +228,26 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
       float amax = 0.f;
       for (int cb = 0; cb < ncb; ++cb) {
 #pragma unroll
-        for (int q = 0; q < 4; ++q) amax = fmaxf(amax, fmaxf(fmaxf(fabsf(cur[q].x), fabsf(cur[q].y)), fmaxf(fabsf(cur[q].z), fabsf(cur[q].w))));
+        for (int q = 0; q < 2; ++q) amax = fmaxf(amax, fmaxf(fmaxf(fabsf(cur[q].x), fabsf(cur[q].y)), fmaxf(fabsf(cur[q].z), fabsf(cur[q].w))));
         if (cb + 1 < ncb) load_blk(cb + 1, nxt);
         mbar_wait(BAR(B_AEMPTY + as), aph ^ 1);
         uint8_t* base = smem + SM_A + as * A_BUF_BYTES;
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {  // two 8-feature chunks of this thread's 16 floats
-          const float4 v0 = cur[2 * c], v1 = cur[2 * c + 1];
-          uint32_t p0[4], p1[4];
-          split2(v0.x, v0.y, p0[0], p1[0]);
-          split2(v0.z, v0.w, p0[1], p1[1]);
-          split2(v1.x, v1.y, p0[2], p1[2]);
-          split2(v1.z, v1.w, p0[3], p1[3]);
-          const int kc = hf * 2 + c;
-          const size_t off = (size_t)(kc * RWP + row) * 16;
-          *reinterpret_cast<uint4*>(base + off) = make_uint4(p0[0], p0[1], p0[2], p0[3]);
-          *reinterpret_cast<uint4*>(base + A_PLANE_BYTES + off) = make_uint4(p1[0], p1[1], p1[2], p1[3]);
-        }
+        uint32_t p0[4], p1[4];
+        split2(cur[0].x, cur[0].y, p0[0], p1[0]);
+        split2(cur[0].z, cur[0].w, p0[1], p1[1]);
+        split2(cur[1].x, cur[1].y, p0[2], p1[2]);
+        split2(cur[1].z, cur[1].w, p0[3], p1[3]);
+        const size_t off = (size_t)(kc * RWP + row) * 16;
+        *reinterpret_cast<uint4*>(base + off) = make_uint4(p0[0], p0[1], p0[2], p0[3]);
+        *reinterpret_cast<uint4*>(base + A_PLANE_BYTES + off) = make_uint4(p1[0], p1[1], p1[2], p1[3]);
         fence_proxy_async();
         mbar_arrive(BAR(B_AFULL + as));
         if (++as == A_BUFS) { as = 0; aph ^= 1; }
 #pragma unroll
-        for (int q = 0; q < 4; ++q) cur[q] = nxt[q];
+        for (int q = 0; q < 2; ++q) cur[q] = nxt[q];
       }
       range_note(amax);
     }
-  } else {
-    // ================================================================ epilogue (4 warps; lane = out feature)
-    const int ew = warp & 3;
-    const int M_ = a.M, Nf_ = a.Nf, act_ = a.act;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int cob = tile / n_tq, tq = tile % n_tq;
-      const int buf = it & 1;
-      const int n = cob * TMF + ew * 32 + lane;
-      const bool nok = n < Nf_;
-      const float bias = (a.bias && nok) ? a.bias[n] : 0.f;
-      const int m0 = tq * TNT;
-      mbar_wait(BAR(B_TFULL + buf), (it >> 1) & 1);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c0 = 0; c0 < TNT; c0 += 32) {
-        float v[32];
-        {
-          float vl[32];
-          tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(buf * 2 * TNT + c0), v);
-          tmem_ld32(tmem_base + ((uint32_t)(ew * 32) << 16) + (uint32_t)(buf * 2 * TNT + TNT + c0), vl);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = fmaf(vl[j], LO_UNSCALE, v[j]);
-        }
-        float rv[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int m = m0 + c0 + j;
-          rv[j] = (a.R && nok && m < M_) ? a.R[(long long)m * a.ldr + n] : 0.f;
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int m = m0 + c0 + j;
-          float val = v[j] + bias;
-          if (act_ == ST2_ACT_GELU) val = gelu_erf(val);
-          else if (act_ == ST2_ACT_TANH) val = tanhf(val);
-          else if (act_ == ST2_ACT_GELU_TANH) val = gelu_tanh(val);
-          val += rv[j];
-          if (nok && m < M_) a.C[(long long)m * a.ldc + n] = val;
-        }
-      }
-      tc_fence_before();
-      mbar_arrive(BAR(B_TEMPTY + buf));
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
   }
 }
 

@@ -98,7 +98,7 @@ __global__ void __launch_bounds__(LSTM_UT* LSTM_BT) lstm_step_kernel(
 
 // Persistent variant: ONE cooperative launch for the whole sequence.  Each CTA keeps its 16 W_hh rows in shared
 // memory for all steps (no per-step re-staging, no per-step launch); the previous hidden state is exchanged through
-// L2 with one grid-wide barrier per step (cooperative groups grid.sync()).  grid = (H/4, 2 directions) <= 148 CTAs.
+// L2 with one grid-wide barrier per step (cooperative groups grid.sync()).  grid = (H/4, 2 directions) <= 132 CTAs.
 __global__ void __launch_bounds__(LSTM_UT* LSTM_BT) lstm_persistent_kernel(
     const float* __restrict__ gx, const float* __restrict__ whh, float* __restrict__ out, long long o_bs, long long o_ts,
     long long o_cs, const int* __restrict__ lengths, int B, int L, int H, float* __restrict__ h0, float* __restrict__ h1,
@@ -270,7 +270,7 @@ __device__ __forceinline__ void lc_mbar_wait(uint32_t bar, uint32_t parity) {
 constexpr int LC_H = 256, LC_CTAS = 8, LC_THREADS = 512, LC_GMAX = 8;
 
 // BG utterances per pass (1..4), `npass` (1 or 2) passes per step: a cluster serves up to 8 utterances so that all
-// clusters of a call are co-resident (a B200 holds ~15 clusters of 8 CTAs; a second wave would double the time).
+// clusters of a call are co-resident (the occupancy query below says how many 8-CTA clusters fit; a second wave would double the time).
 template <int BG>
 __global__ void __cluster_dims__(LC_CTAS, 1, 1) __launch_bounds__(LC_THREADS, 1)
     lstm_cluster_kernel(const float* __restrict__ gx, const float* __restrict__ whh, float* __restrict__ out, long long o_bs,
@@ -289,7 +289,7 @@ __global__ void __cluster_dims__(LC_CTAS, 1, 1) __launch_bounds__(LC_THREADS, 1)
   const int nlive = min(gsize, B - b0);
   const uint32_t fill_bytes = (uint32_t)nlive * H * 4u;     // 8 CTAs x 32 units x nlive utterances x 4 B
 
-  // W_hh rows of unit j, 4 gates, this thread's 16 k's, as (even k, odd k) pairs for the packed FFMA2 pipe
+  // W_hh rows of unit j, 4 gates, this thread's 16 k's, as (even k, odd k) pairs (two independent FMA chains)
   float2 w[4][8];
 #pragma unroll
   for (int g = 0; g < 4; ++g) {
@@ -363,8 +363,10 @@ __global__ void __cluster_dims__(LC_CTAS, 1, 1) __launch_bounds__(LC_THREADS, 1)
             const float2 h01 = make_float2(hv.x, hv.y), h23 = make_float2(hv.z, hv.w);
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
-              acc[bb][g] = __ffma2_rn(h01, w[g][q * 2 + 0], acc[bb][g]);
-              acc[bb][g] = __ffma2_rn(h23, w[g][q * 2 + 1], acc[bb][g]);
+              acc[bb][g].x = fmaf(h01.x, w[g][q * 2 + 0].x, acc[bb][g].x);
+              acc[bb][g].y = fmaf(h01.y, w[g][q * 2 + 0].y, acc[bb][g].y);
+              acc[bb][g].x = fmaf(h23.x, w[g][q * 2 + 1].x, acc[bb][g].x);
+              acc[bb][g].y = fmaf(h23.y, w[g][q * 2 + 1].y, acc[bb][g].y);
             }
           }
         }
@@ -451,7 +453,7 @@ extern "C" int st2_lstm_bidir(const float* gx, const float* whh, float* out, lon
   ST2_REQUIRE(gx && whh && out && work && B > 0 && L > 0 && H > 0 && H % 4 == 0, "st2_lstm_bidir", "bad args");
   cudaStream_t st = (cudaStream_t)stream;
   if (H == LC_H && g_lstm_cluster) {
-    // how many 8-CTA clusters the device holds at once (GPC geometry: ~15 on a B200); a second wave would double the time
+    // how many 8-CTA clusters the device holds at once (GPC geometry); a second wave would double the time
     static int max_clusters = 0;
     if (max_clusters == 0) {
       cudaLaunchConfig_t cfg = {};

@@ -141,7 +141,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -m styletts2_b200.build` "
-            "(nvcc -gencode arch=compute_100a,code=sm_100a). There is no CPU fallback.")
+            "(nvcc -gencode arch=compute_90a,code=sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)  # AttributeError if the symbol is not exported

@@ -72,7 +72,7 @@ class WNConv1d(_Cached):
 
 
 def _maybe_wtc(w, stride, dilation, mode=TC_FAST):
-    """plane-split tensor-core weight blocks when the tcgen05 conv supports the shape and it is worth it.
+    """plane-split tensor-core weight blocks when the wgmma conv supports the shape and it is worth it.
     mode: precision recipe (TC_FAST for the decoder / vocoder, TC_ACCURATE for the F0/N predictor)."""
     co, ci, k = w.shape
     # Cout < 16 (conv_post of HiFi-GAN: one output channel) only through the time-major kernel, whose N is Cout rounded up to 16
@@ -164,7 +164,7 @@ class WNConvTranspose1d(_Cached):
 
 
 class Linear(nn.Linear):
-    """nn.Linear whose forward is the GEMM kernel (fp32 SIMT for small row counts, fp32-accurate tcgen05 otherwise)."""
+    """nn.Linear whose forward is the GEMM kernel (fp32 SIMT for small row counts, fp32-accurate wgmma otherwise)."""
 
     def _wtc(self):
         k = (self.weight.data_ptr(), self.weight._version, str(self.weight.device))

@@ -72,6 +72,11 @@ def stats_parts(lq: int) -> int:
     return (lq + 255) // 256
 
 
+def tc_stats_parts(lq: int) -> int:
+    """InstanceNorm partials of the tensor-core conv kernels: one per 64-frame tile."""
+    return (lq + 63) // 64
+
+
 def _fill_conv_args(a: ConvArgs, x, wt, bias, y, *, K, stride, dil, pad, Lq, y_len, pre, pre_act, slope, alpha, res,
                     res_shift, out_div, accum_mode, accum_div, out_act, stats, nparts):
     B, Cin, Lin = x.shape
@@ -125,7 +130,7 @@ class _prof:
 
 
 CONVT_PHASE_MAJOR = os.environ.get("ST2_CONVT_PHASE_MAJOR", "1") != "0"   # tensor-core ConvTranspose through a phase-major scratch buffer
-USE_TC = os.environ.get("ST2_TC", "1") != "0"   # tensor-core (tcgen05) conv path where a wtc buffer is given
+USE_TC = os.environ.get("ST2_TC", "1") != "0"   # tensor-core (wgmma) conv path where a wtc buffer is given
 TC_MIN_WORK = 1 << 22                            # below this many MACs per utterance the SIMT kernel is used
 
 
@@ -171,7 +176,7 @@ def conv1d(x, wt, bias=None, *, K, stride=1, dil=1, pad=0, pre=None, pre_act=ACT
            res=None, res_shift=0, out_div=1.0, accum_mode=0, accum_div=1.0, out_act=ACT_NONE, out=None,
            want_stats=False, wtc=None, tc_max_ctas=0) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Fused Conv1d (see include/styletts2_b200.h).  wt is the [Cin,K,Cout] layout.
-    wtc: optional tensor-core weight buffer (conv_tc_weight_layout) -> tcgen05 path when supported.
+    wtc: optional tensor-core weight buffer (conv_tc_weight_layout) -> wgmma path when supported.
     Returns (y [B,Cout,Lout], stats [B,Cout,nparts,3] or None)."""
     x = _cl(x)
     B, Cin, Lin = x.shape
@@ -182,7 +187,7 @@ def conv1d(x, wt, bias=None, *, K, stride=1, dil=1, pad=0, pre=None, pre_act=ACT
         out = empty(B, Cout, Lout, device=x.device)
     assert out.shape == (B, Cout, Lout) and out.stride(2) == 1 and out.stride(1) == Lout
     use_tc = wtc is not None and USE_TC and stride == 1 and Cin * Cout * K * Lout >= TC_MIN_WORK
-    nparts = stats_parts(Lout) * (2 if use_tc else 1)
+    nparts = tc_stats_parts(Lout) if use_tc else stats_parts(Lout)
     stats = empty(B, Cout, nparts, 3, device=x.device) if want_stats else None
     a = ConvArgs()
     _fill_conv_args(a, x, wt, bias, out, K=K, stride=stride, dil=dil, pad=pad, Lq=Lout, y_len=Lout, pre=pre,
@@ -235,7 +240,7 @@ def conv_transpose1d(x, wp, bias, *, K, stride, padding, pre_act=ACT_NONE, slope
     phase_major = use_tc and CONVT_PHASE_MAJOR and out.stride(2) == 1 and out.stride(1) == Lout
     if use_tc and not phase_major and (wtc.mode & TC_TMAJOR):
         use_tc = False   # the direct (strided-store) variant has no time-major kernel: FP32-pipe path
-    nparts = 1 if phase_major else S * stats_parts(Lin) * (2 if use_tc else 1)
+    nparts = 1 if phase_major else S * (tc_stats_parts(Lin) if use_tc else stats_parts(Lin))
     stats = empty(B, Cout, nparts, 3, device=x.device) if want_stats else None
     a = ConvArgs()
     _fill_conv_args(a, x, wp, bias, out, K=1, stride=1, dil=1, pad=0, Lq=Lin, y_len=Lout, pre=None, pre_act=pre_act,
@@ -357,7 +362,7 @@ def linear_tc_weight_layout(W: torch.Tensor) -> torch.Tensor:
 
 def linear(A, W, bias=None, *, act=ACT_NONE, R=None, out=None, wtc=None):
     """A [..., K] @ W[Nf,K]^T (+bias, act, +R) -> [..., Nf].  Rows may be strided (ld).
-    wtc: optional tensor-core weight blocks (linear_tc_weight_layout) -> fp32-accurate tcgen05 path for big M."""
+    wtc: optional tensor-core weight blocks (linear_tc_weight_layout) -> fp32-accurate wgmma path for big M."""
     K = A.shape[-1]
     A2, M, lda = _rows_view(A)
     Nf = W.shape[0]
@@ -407,13 +412,13 @@ def linear_strided(x, B, Lr, K, bs, ls, ks, W, bias=None, *, act=ACT_NONE, out=N
     return out
 
 
-ATT_TC = os.environ.get("ST2_ATT_TC", "1") != "0"   # tcgen05 attention (fp32-accurate) where supported
+ATT_TC = os.environ.get("ST2_ATT_TC", "1") != "0"   # wgmma attention (fp32-accurate) where supported
 ATT_TC_MIN_N = 32
 
 
 def attention_ex(q, k, v, out, B, N, H, D, lengths=None):
     """softmax(q k^T / sqrt(D)) v per (utterance, head).  q / k / v / out: 2-D row views [B*N, >= H*D] (row strides free,
-    head h in columns h*D..); lengths (int32 [B]) = key-padding mask.  tcgen05 kernel when the layout allows it."""
+    head h in columns h*D..); lengths (int32 [B]) = key-padding mask.  wgmma kernel when the layout allows it."""
     scale = float(D) ** -0.5
     use_tc = (ATT_TC and USE_TC and N >= ATT_TC_MIN_N and k.stride(0) == v.stride(0)
               and bool(L.load().st2_attention_tc_supported(q.stride(0), k.stride(0), out.stride(0), D))

@@ -4,7 +4,7 @@ The reference wraps `transformers.AlbertModel` and returns `last_hidden_state` (
 config is Utils/PLBERT/config.yml:23-30 (vocab 178, hidden 768, 12 heads, intermediate 2048, 12 layers sharing ONE
 set of weights, embedding size 128, gelu_new, LayerNorm eps 1e-12).  This module keeps AlbertModel's state-dict keys
 (so `load_plbert`'s stripped checkpoint loads unchanged) and its call `bert(tokens, attention_mask=(~text_mask).int())`.
-Its output feeds the duration path, so every GEMM runs at fp32 accuracy (SIMT fp32 or the 3-plane tcgen05 GEMM).
+Its output feeds the duration path, so every GEMM runs at fp32 accuracy (SIMT fp32 or the 3-plane wgmma GEMM).
 """
 from __future__ import annotations
 

@@ -1,4 +1,4 @@
-"""GPU tier: the tcgen05 attention kernel (csrc/attention_tc.cu: QK^T and PV on the tensor cores, S / O in TMEM, fp16
+"""GPU tier: the wgmma attention kernel (csrc/attention_tc.cu: QK^T and PV on the tensor cores, S / O in registers, fp16
 two-plane split with separate correction accumulators) against a float64 reference, next to the fp32 SIMT kernel: the
 durations are downstream of the denoiser, so the bar is fp32 accuracy (modules.py:523-535; PL-BERT key-padding mask)."""
 import pytest

@@ -1,4 +1,4 @@
-"""GPU tier: the tcgen05 / TMEM tensor-core Conv1d against fp32 torch, for each precision recipe (csrc/conv_tc.cu):
+"""GPU tier: the wgmma tensor-core Conv1d against fp32 torch, for each precision recipe (csrc/conv_tc.cu):
 FAST (fp16 high planes + one e4m3 K=32 correction MMA; ~2^-16 per product), ACCURATE (two fp16 planes, separate
 correction accumulator; fp32-SIMT level) and F16X3 (the accurate planes in one accumulator).  Tolerances relative to the
 output scale; a single 16-bit pass would be ~1e-3."""
@@ -29,7 +29,7 @@ TC_CASES = [
     (2, 256, 256, 11, 5, 1300, 0),   # two co blocks, max window
     (3, 64, 64, 7, 5, 2000, 0),      # Cout padded to 128
     (2, 48, 32, 11, 1, 900, 0),      # Cin, Cout padded
-    (4, 128, 128, 3, 1, 3000, 5),    # persistent loop: 48 tiles on 5 CTAs (TMEM double buffering, phase wrap)
+    (4, 128, 128, 3, 1, 3000, 5),    # persistent loop on 5 CTAs (stage ring phase wrap)
     (3, 128, 128, 7, 1, 1201, 0),    # odd row length: every channel row starts at a different 4-byte phase (16-byte cp.async windows)
     (2, 22, 128, 1, 1, 2403, 0),     # Cin not a multiple of 16 (zero-filled channels), odd length
     (2, 80, 256, 3, 5, 515, 3),      # odd length, tail tile, few CTAs

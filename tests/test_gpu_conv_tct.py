@@ -36,12 +36,12 @@ TCT_CASES = [
     (2, 32, 32, 11, 1, 2000, 0),     # HiFi-GAN C=32 stage
     (2, 32, 32, 11, 5, 1531, 0),     # max window, odd length
     (3, 64, 64, 7, 3, 2000, 0),      # HiFi-GAN C=64 stage
-    (2, 64, 64, 3, 1, 4099, 4),      # persistent loop on 4 CTAs (TMEM double buffering, barrier phase wrap), odd length
+    (2, 64, 64, 3, 1, 4099, 4),      # persistent loop on 4 CTAs (barrier phase wrap), odd length
     (2, 128, 22, 7, 1, 1201, 0),     # conv_post of iSTFTNet (Cout 22 -> 32 rows)
     (2, 32, 1, 7, 1, 3000, 0),       # conv_post of HiFi-GAN (Cout 1 -> 16 rows)
     (2, 48, 16, 3, 1, 700, 0),       # N = 16
     (2, 80, 96, 3, 5, 515, 3),       # N = 96 (3 channel groups), tail tile
-    (2, 128, 128, 3, 1, 1500, 0),    # N = 128: TMEM fully used (2 buffers x 2 M blocks x 128 columns)
+    (2, 128, 128, 3, 1, 1500, 0),    # N = 128: widest accumulator (two warpgroups x 64 channels)
     (3, 128, 128, 7, 1, 1201, 5),
     (2, 22, 128, 1, 1, 2403, 0),
     (1, 64, 64, 7, 1, 100, 0),       # single partial tile: M block 1 entirely beyond the row

@@ -252,7 +252,7 @@ def test_end_to_end_matches_live_oracle_ragged_free_batch():
 def test_sharded_batch_equals_single_batch_bitwise():
     """Utterance sharding (SURVEY section 8e): running utterances [0:2] and [2:4] separately gives bit-identical
     waveforms to running [0:4] together (no cross-utterance op; deterministic reductions).  The GEMM variant is picked
-    from the row count (<= 64 rows: weight-streaming kernel, < 256: fp32 tile SGEMM, >= 256: tcgen05), each with its own
+    from the row count (<= 64 rows: weight-streaming kernel, < 256: fp32 tile SGEMM, >= 256: wgmma), each with its own
     summation order, so the property holds whenever both runs fall in the same regimes -- as here (token rows 512 / 256,
     frame rows 1536 / 768, per-utterance rows 4 / 2) and in any weak-scaling deployment (same per-GPU batch on every rank)."""
     from styletts2_b200.inference import Synthesizer
