@@ -210,9 +210,10 @@ int st2_linear_tc(const float* A, long long lda, const void* wtc, const float* b
  * (st2_linear_tc_split_bytes bytes): both operands then reach shared memory by 1-D TMA bulk copies and no warp spends
  * issue slots on conversion (the on-the-fly path re-splits the same rows once per 128-feature output block).
  * planes == NULL falls back to on-the-fly splitting of A. */
-/* Range guard of the fp16-plane GEMM: *flag_out = 1 if any activation or weight split since the last call had
- * |x| >= 65504 (or was NaN) -- the result of that GEMM is then inf/NaN, not silently wrong; the flag is cleared.
- * Synchronises with the device (call it after a pass, outside CUDA-graph capture). */
+/* Range guard of the fp16-plane GEMM and tensor-core convs: *flag_out = 1 if any operand split since the last call left
+ * fp16's range or was NaN -- GEMM activations / weights with |x| >= 65504, conv operands after their power-of-two scales
+ * (|z| >= 65504 / 64 after the prologue, |w| >= 65504 / 4096) -- the result of that GEMM / conv is then inf/NaN, not
+ * silently wrong; both flags are cleared.  Synchronises with the device (call it after a pass, outside CUDA-graph capture). */
 int st2_range_flag_fetch(int* flag_out);
 long long st2_linear_tc_split_bytes(int M, int K);
 int st2_linear_tc_split(const float* A, long long lda, int M, int K, void* planes, void* stream);

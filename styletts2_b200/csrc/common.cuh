@@ -13,6 +13,9 @@ namespace st2 {
 void set_error(const char* where, cudaError_t e);
 void set_error_msg(const char* where, const char* msg);
 
+// Range flag of the tensor-core convs (conv_tc.cu): reads and clears it; st2_range_flag_fetch reports it with the GEMMs' flag.
+cudaError_t conv_tc_range_flag_fetch(int* flag);
+
 #define ST2_CHECK_LAUNCH(where)                         \
   do {                                                  \
     cudaError_t _e = cudaGetLastError();                \

@@ -85,6 +85,14 @@ constexpr float W_SCALE = 4096.0f, X_SCALE = 64.0f, D_UNSCALE = 1.0f / (4096.0f 
 constexpr float ACC_LO_SCALE = 256.0f, ACC_LO_UNSCALE = 1.0f / 256.0f;            // ST2_TC_ACCURATE low planes
 constexpr float F8_WLO = 16.0f, F8_WHI = 1.0f / 256.0f, F8_XHI = 1.0f / 16.0f, F8_XLO = 256.0f;  // e4m3 correction operands
 
+// Range guard (as in linear_tc.cu, with a flag of its own): the fp16 high planes hold |z'| = 64 |z| and |w'| = 4096 |w| below
+// 65504, i.e. |z| < 1023.5 after the prologue and |w| < 16; beyond that (or for NaN) the conv writes inf/NaN.  Every stager
+// thread keeps one predicate over the rows it converts and raises the flag once; the weight layout kernels check the weights.
+// st2_range_flag_fetch() reports and clears it.  Not covered: the FAST recipe's e4m3 corrections saturate (silently, to
+// +-448) from |z| of about 64 on (DESIGN.md "Precision recipes").
+__device__ int g_range_flag = 0;
+constexpr float FP16_MAX = 65504.0f;
+
 constexpr int SM_W = 0;
 constexpr int SM_ACT = SM_W + W_STAGES * W_STAGE_BYTES;
 constexpr int SM_RAW = SM_ACT + 2 * ACT_BUF_BYTES;
@@ -129,7 +137,7 @@ __device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cas
 template <int ACT, int MODE>
 __device__ __forceinline__ void stage_row(const float (&x)[8], const float (&pa)[8], const float (&pb)[8], const float (&al)[8],
                                           const float (&ia)[8], float slope, bool inb, uint8_t* p0, uint8_t* p1, int kc, int r,
-                                          int RWP) {
+                                          int RWP, bool& in_range) {
   float v[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -141,6 +149,7 @@ __device__ __forceinline__ void stage_row(const float (&x)[8], const float (&pa)
       z = z > 0.f ? z : z * slope;
     }
     v[j] = inb ? z : 0.f;  // zero padding applies AFTER the activation
+    in_range = in_range && fabsf(v[j]) < FP16_MAX;   // false for NaN too
   }
   uint32_t hp[4];
   float lo[8];
@@ -296,6 +305,7 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
   constexpr int NRC = (RW_MAX + ROWS_PER_PASS - 1) / ROWS_PER_PASS;
   const float xs_ = X_SCALE;
   int cb = 0, c_slot = 0;
+  bool in_range = true;   // range guard: every operand this thread converted is below FP16_MAX
   unsigned c_row0 = 0;   // low 32 bits of the element index of (tile's utterance, channel 0, first window frame): only its 4-byte phase is used
   for (int g = 0; g < total_blocks; ++g) {
     if (cb == 0) {
@@ -350,9 +360,9 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
         float xv[8];
 #pragma unroll
         for (int j = 0; j < 8; ++j) xv[j] = raw[sh[j] + r];
-        if (pre_act_ == ST2_ACT_SNAKE) stage_row<ST2_ACT_SNAKE, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP);
-        else if (pre_act_ == ST2_ACT_LRELU) stage_row<ST2_ACT_LRELU, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP);
-        else stage_row<ST2_ACT_NONE, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP);
+        if (pre_act_ == ST2_ACT_SNAKE) stage_row<ST2_ACT_SNAKE, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP, in_range);
+        else if (pre_act_ == ST2_ACT_LRELU) stage_row<ST2_ACT_LRELU, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP, in_range);
+        else stage_row<ST2_ACT_NONE, MODE>(xv, pa, pb, al, ia, slope_, inb, p0, p1, kc, r, RWP, in_range);
       }
     }
     fence_proxy_async();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
@@ -362,6 +372,7 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
     if (++c_slot == RAW_STAGES) c_slot = 0;
   }
   asm volatile("cp.async.wait_group 0;" ::: "memory");
+  if (!in_range) atomicExch(&g_range_flag, 1);
 }
 
 // Release bookkeeping of the consumer warpgroups: the MMAs of one weight stage are committed as one wgmma group and at most
@@ -780,6 +791,14 @@ __device__ __forceinline__ void weight_stage_store(uint8_t* blk, int byte_in_sta
   }
 }
 
+// Range guard of the weights: w' = w * 2^12 must fit the fp16 high plane (NaN fails the compare too).
+__device__ __forceinline__ void weight_range_note(const float (&wr)[16]) {
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) ok = ok && fabsf(wr[j] * W_SCALE) < FP16_MAX;
+  if (!ok) atomicExch(&g_range_flag, 1);
+}
+
 // Row `col` of output-channel block `cob` -> output channel (or -1): rows are the channels of the block in order (the
 // time-major layout has one block of NC rows).
 __device__ __forceinline__ int weight_row_channel(int Cout, int cob, int col, bool tmajor) {
@@ -808,6 +827,7 @@ __global__ void conv_tc_weight_layout_kernel(const float* __restrict__ w, uint8_
       const int ci = cb * CB + j;
       wr[j] = (co >= 0 && ci < Cin) ? w[((long long)co * Cin + ci) * K + tap] : 0.f;
     }
+    weight_range_note(wr);
     uint8_t* blk = out + (((long long)cob * ncb + cb) * K + tap) * step_bytes;
     const int base = plane * (KCB * rows * 16) + (chunk * rows + col) * 16;
 #pragma unroll
@@ -838,6 +858,7 @@ __global__ void convT_tc_weight_layout_kernel(const float* __restrict__ w, uint8
       const int ci = cb * CB + j;
       wr[j] = (co >= 0 && ci < Cin && kk < K) ? w[((long long)ci * Cout + co) * K + kk] : 0.f;
     }
+    weight_range_note(wr);
     uint8_t* blk = out + ((long long)ph * J * n_cob * ncb + ((long long)cob * ncb + cb) * J + kp) * step_bytes;
     const int base = plane * (KCB * rows * 16) + (chunk * rows + col) * 16;
 #pragma unroll
@@ -953,6 +974,15 @@ static int launch_tc(const st2_conv_args& a, const void* wtc, int mode, int max_
 }
 
 }  // namespace tc
+
+cudaError_t conv_tc_range_flag_fetch(int* flag) {
+  int v = 0, zero = 0;
+  cudaError_t e = cudaMemcpyFromSymbol(&v, tc::g_range_flag, sizeof(int));   // synchronises with the device
+  if (e == cudaSuccess && v) e = cudaMemcpyToSymbol(tc::g_range_flag, &zero, sizeof(int));
+  *flag = v;
+  return e;
+}
+
 }  // namespace st2
 
 using namespace st2;

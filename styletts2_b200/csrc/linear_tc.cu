@@ -326,8 +326,10 @@ int st2_range_flag_fetch(int* flag_out) {
   int v = 0, zero = 0;
   cudaError_t e = cudaMemcpyFromSymbol(&v, ltc::g_range_flag, sizeof(int));     // synchronises with the device
   if (e == cudaSuccess && v) e = cudaMemcpyToSymbol(ltc::g_range_flag, &zero, sizeof(int));
+  int vc = 0;
+  if (e == cudaSuccess) e = conv_tc_range_flag_fetch(&vc);                       // the tensor-core convs' flag (conv_tc.cu)
   if (e != cudaSuccess) { set_error("st2_range_flag_fetch", e); return (int)e; }
-  *flag_out = v;
+  *flag_out = v | vc;
   return 0;
 }
 

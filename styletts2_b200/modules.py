@@ -691,6 +691,12 @@ class Decoder(nn.Module):
         self.F0_conv = WNConv1d(1, 1, 3, stride=2, padding=1)
         self.N_conv = WNConv1d(1, 1, 3, stride=2, padding=1)
         self.asr_res = nn.Sequential(WNConv1d(512, 64, 1))
+        # The learned shortcut 1x1 convs read the cat buffers raw (no AdaIN in front), and one of their input channels is
+        # F0_conv(F0 in Hz): a trained F0_conv puts 60..400 there, past the FAST recipe's envelope (its e4m3 corrections
+        # saturate from |z| ~ 64 on and it falls to single-fp16 accuracy, ~4e-4).  ACCURATE keeps fp32-level accuracy up to
+        # the fp16 range; these convs have K = 1 and run at the token-frame rate, so the third MMA costs little.
+        for blk in [self.encode, *self.decode]:
+            set_tc_mode(blk.conv1x1, TC_ACCURATE)
         if gen_istft_n_fft is not None:
             self.generator = Generator(style_dim, resblock_kernel_sizes, upsample_rates, upsample_initial_channel,
                                        resblock_dilation_sizes, upsample_kernel_sizes, gen_istft_n_fft, gen_istft_hop_size)

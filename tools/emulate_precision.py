@@ -1,7 +1,9 @@
 """Precision recipes of the tensor-core conv, EMULATED on the CPU oracle before any kernel was written (decision record):
 every convolution / transposed convolution of the decoder that runs on the tensor-core kernel (stride 1, >= 16 channels) is
 replaced by the arithmetic of a recipe; the waveform is compared with the exact fp32 oracle on the two decoder cases of
-oracle/cases.py.    python tools/emulate_precision.py > profiles/r02_precision_emulation.txt   (build container, ~1 min)"""
+oracle/cases.py.  The shipped recipes (FAST, ACCURATE, F16X3) come from oracle/tc_recipes.py, the recipe-exact reference of
+the kernel's operand rounding (float64 plane products); the rejected ones are plain fp32 emulations.
+    python tools/emulate_precision.py        (CPU, a few minutes)"""
 import os
 import sys
 
@@ -13,14 +15,11 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):
     sys.path.insert(0, p)
 import cases  # noqa: E402
 import styletts2_oracle as O  # noqa: E402
+import tc_recipes as R  # noqa: E402
 from util import oracle_sds  # noqa: E402
 
 oc, oct_ = F.conv1d, F.conv_transpose1d
-f8 = torch.float8_e4m3fn
-
-
-def q8(t):
-    return t.to(f8).float()
+SHIPPED = {"FAST": R.FAST, "ACCURATE": R.ACCURATE, "F16X3": R.F16X3}
 
 
 def split16(t):
@@ -37,15 +36,8 @@ def recipe_conv(fn, x, w, kw, mode):
     if mode == "bf16_hi_lo_x3":                 # round 1
         xb = x.bfloat16().float(); xl = (x - xb).bfloat16().float(); wb = w.bfloat16().float(); wl = (w - wb).bfloat16().float()
         return fn(xb, wb, None, **kw) + fn(xl, wb, None, **kw) + fn(xb, wl, None, **kw)
-    if mode == "fp16_two_planes_x3":            # ACCURATE / F16X3 planes
-        xh, xl = split16(x); wh, wl = split16(w)
-        return fn(xh, wh, None, **kw) + fn(xl.half().float(), wh, None, **kw) + fn(xh, wl.half().float(), None, **kw)
-    if mode == "FAST_fp16_plus_e4m3_corrections":   # the shipped recipe, with its power-of-two scalings
-        xs, ws = x * 64.0, w * 4096.0
-        xh, xl = split16(xs); wh, wl = split16(ws)
-        main = fn(xh, wh, None, **kw)
-        corr = fn(q8(xh / 16.0), q8(wl * 16.0), None, **kw) + fn(q8(xl * 256.0), q8(wh / 256.0), None, **kw)
-        return (main + corr) / (64.0 * 4096.0)
+    if mode in SHIPPED:                         # the kernel's recipes, operand rounding reproduced exactly
+        return R.recipe_conv(fn, x, w, SHIPPED[mode], **kw).to(x.dtype)
     raise ValueError(mode)
 
 
@@ -85,9 +77,10 @@ def run(name, mode):
 
 if __name__ == "__main__":
     torch.set_num_threads(8)
-    print("# waveform max-abs error of the whole decoder when every tensor-core conv uses the recipe (CPU emulation, fp32 accumulate)")
+    print("# waveform max-abs error of the whole decoder when every tensor-core conv uses the recipe (CPU emulation; fp32 accumulation"
+          " for the rejected recipes, float64 for the shipped ones)")
     for name in ("lj_dec", "libri_dec"):
         ref = run(name, "exact")
-        for mode in ("tf32_like_fp16_both", "fp16_weights_x_two_planes", "bf16_hi_lo_x3", "fp16_two_planes_x3", "FAST_fp16_plus_e4m3_corrections"):
+        for mode in ("tf32_like_fp16_both", "fp16_weights_x_two_planes", "bf16_hi_lo_x3", *SHIPPED):
             o = run(name, mode)
             print(f"{name:10s} {mode:34s} max-abs {float((o - ref).abs().max()):.3e}   (waveform scale {float(ref.abs().max()):.2f})", flush=True)
