@@ -126,8 +126,8 @@ int st2_conv1d_tc(const st2_conv_args* a, const void* wtc, int mode, int max_cta
 /* Profiling aid: when set to a device buffer of 4*16*8 int64, CTA 0 of st2_conv1d_tc records per-role cycle
  * counters for its first 16 tiles (role 0 MMA, 1 weight producer, 2 stagers, 3 epilogue); NULL disables. */
 int st2_debug_set_trace(void* buf);
-/* Timing experiments only (tools/tc_bench.py): bit 0 second FAST MMA as kind::f16, bit 1 epilogue without global
- * traffic, bit 2 stagers skip the conversion, bit 3 no MMAs.  Results are wrong while any bit is set; 0 restores. */
+/* Timing experiments only (tools/conv_tc_shapes.py --ablate), tensor-core convs: 4 stagers skip the conversion,
+ * 16 no weight copies, 32 no raw activation copies.  Results are wrong while any bit is set; 0 restores. */
 int st2_debug_set_flags(int flags);
 /* Polyphase ConvTranspose1d on the same tensor-core kernel (one launch per phase); wtc from
  * st2_convT_tc_weight_layout (st2_convT_tc_weight_bytes bytes).  Arguments as st2_conv_transpose1d. */

@@ -58,7 +58,7 @@ constexpr int W_PLANE_BYTES = KCB * TM * 16;    // 4 KB
 constexpr int W_STEP_BYTES = 2 * W_PLANE_BYTES; // one (16 ci, tap) step: plane 0 (fp16 high) | plane 1 (fp8 corrections or fp16 low) = 8 KB
 constexpr int TPS = 2;                          // taps per pipeline stage: one wait / one commit / one bulk copy per 2 taps (the
                                                 // per-stage handshake of the two single-thread roles costs ~300 cycles, as much
-                                                // as the 2 MMAs of one tap: profiles/r02_tc_bench_*.txt)
+                                                // as the 2 MMAs of one tap)
 constexpr int W_STAGE_BYTES = TPS * W_STEP_BYTES;  // 16 KB
 constexpr int W_STAGES = 3;                     // 48 KB (6 taps) of weights in flight per SM
 constexpr int RW_MAX = 312;                     // TN + (K-1)*dil rounded up to 8, max
@@ -107,7 +107,7 @@ static_assert(SM_TOTAL <= 232448, "shared memory budget (227 KB per CTA)");
 constexpr int B_WFULL = 0, B_WEMPTY = W_STAGES, B_AFULL = 2 * W_STAGES, B_AEMPTY = B_AFULL + 2, B_COUNT = B_AFULL + 4;
 static_assert(8 * B_COUNT + 8 <= 512, "barrier area");
 
-// Timing-experiment switches (tools/tc_bench.py; results are WRONG when any is set; 0 in production):
+// Timing-experiment switches (tools/conv_tc_shapes.py --ablate; results are WRONG when any is set; 0 in production):
 //   4 = stagers skip the conversion (stale operands), 16 = no weight copies, 32 = no raw activation copies
 __device__ int g_dbg = 0;
 __device__ long long* g_trace = nullptr;   // reserved for per-role cycle traces (st2_debug_set_trace); unused by these kernels
@@ -127,6 +127,11 @@ __device__ __forceinline__ TileCoord tile_coord(int tile, int n_tq, int n_cob) {
 }
 
 __device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+
+// Warp index broadcast from lane 0, so that ptxas can prove it warp-uniform.  With a plain tid >> 5 it treats the consumer
+// branch of the role dispatch as divergent and serializes every wgmma behind a full drain (ptxas C7520), which also
+// defeats the one-group-in-flight pipeline of the consumer loops.
+__device__ __forceinline__ int warp_uniform(int tid) { return __shfl_sync(0xffffffffu, tid >> 5, 0); }
 
 // ---------------------------------------------------------------------------------------------
 // Stager inner work for one frame row (8 channels of one K chunk): AdaIN affine + activation (coefficients carry the
@@ -408,7 +413,7 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
   // RW = window rows (TN + (K-1)*dil, rounded up to 8); RWP = chunk pitch in rows
   const int RWP = RW + 2;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = warp_uniform(tid), lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SM_BAR;
   auto BAR = [&](int i) { return bar0 + 8u * i; };
@@ -570,7 +575,8 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
 // warpgroup through shared memory (two passes: mean, then M2).  FAST recipe only.
 __host__ __device__ __forceinline__ int tmajor_nc(int Cout) { return Cout <= 16 ? 16 : ((Cout + 31) & ~31); }
 
-constexpr int T_WSTAGE = 8192;                            // bytes per weight stage: 8 taps (NC = 16) .. 1 tap (NC = 128)
+constexpr int T_WSTAGE = 16384;                           // bytes per weight stage: 16 taps (NC = 16) .. 2 taps (NC = 128)
+static_assert(T_WSTAGE <= W_STAGE_BYTES, "time-major stages live in the SM_W ring");
 
 template <int NH>   // channels per warpgroup = NC / 2
 __device__ __forceinline__ void tct_mma(float (&d)[NH / 2], float (&e)[NH / 2], uint64_t a0, uint64_t b0, uint64_t a1, uint64_t b1,
@@ -590,7 +596,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
   constexpr int NJ = NH / 8;
   const int RWP = RW + 2;
   extern __shared__ __align__(1024) uint8_t smem[];
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = warp_uniform(tid), lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SM_BAR;
   auto BAR = [&](int i) { return bar0 + 8u * i; };
