@@ -210,10 +210,11 @@ int st2_linear_tc(const float* A, long long lda, const void* wtc, const float* b
  * (st2_linear_tc_split_bytes bytes): both operands then reach shared memory by 1-D TMA bulk copies and no warp spends
  * issue slots on conversion (the on-the-fly path re-splits the same rows once per 128-feature output block).
  * planes == NULL falls back to on-the-fly splitting of A. */
-/* Range guard of the fp16-plane GEMM and tensor-core convs: *flag_out = 1 if any operand split since the last call left
- * fp16's range or was NaN -- GEMM activations / weights with |x| >= 65504, conv operands after their power-of-two scales
- * (|z| >= 65504 / 64 after the prologue, |w| >= 65504 / 4096) -- the result of that GEMM / conv is then inf/NaN, not
- * silently wrong; both flags are cleared.  Synchronises with the device (call it after a pass, outside CUDA-graph capture). */
+/* Range guard of the fp16-plane GEMM, attention and tensor-core convs: *flag_out = 1 if any operand split since the last
+ * call left fp16's range or was NaN -- GEMM activations / weights and attention q / k / v with |x| >= 65504, conv operands
+ * after their power-of-two scales (|z| >= 65504 / 64 after the prologue, |w| >= 65504 / 4096) -- the result of that GEMM /
+ * attention / conv is then inf/NaN, not silently wrong; all flags are cleared.  Synchronises with the device (call it
+ * after a pass, outside CUDA-graph capture). */
 int st2_range_flag_fetch(int* flag_out);
 long long st2_linear_tc_split_bytes(int M, int K);
 int st2_linear_tc_split(const float* A, long long lda, int M, int K, void* planes, void* stream);
@@ -229,9 +230,11 @@ int st2_attention(const float* q, const float* kv, float* out, int B, int N, int
 int st2_attention_ex(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out, long long out_ld,
                      const int* lengths, int B, int N, int H, int D, float scale, void* stream);
 /* The same contraction on the tensor cores (wgmma, register accumulators for S and O, fp16 two-plane split with separate
- * correction accumulators = fp32 accuracy; csrc/attention_tc.cu): one CTA per (128 query rows, head, utterance), keys in
+ * correction accumulators = fp32 accuracy; csrc/attention_tc.cu): one CTA per (64 query rows, head, utterance), keys in
  * blocks of 128.  Needs D == 64, row strides that are multiples of 4 floats and 16-byte aligned pointers
- * (st2_attention_tc_supported); arguments as st2_attention_ex. */
+ * (st2_attention_tc_supported); arguments as st2_attention_ex.  Every length must be >= 1: a row with no valid key has
+ * a zero softmax sum and a non-finite output, here and in st2_attention_ex.  q / k / v values that reach the fp16 planes
+ * (valid keys, query rows < N) raise the range flag of st2_range_flag_fetch when |x| >= 65504 or NaN. */
 int st2_attention_tc_supported(long long q_ld, long long kv_ld, long long out_ld, int D);
 int st2_attention_tc(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out, long long out_ld,
                      const int* lengths, int B, int N, int H, int D, float scale, void* stream);

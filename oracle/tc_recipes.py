@@ -1,4 +1,5 @@
-"""Recipe-exact CPU reference of the tensor-core conv (styletts2_b200/csrc/conv_tc.cu).
+"""Recipe-exact references of the tensor-core conv (styletts2_b200/csrc/conv_tc.cu), GEMM (linear_tc.cu) and attention
+(attention_tc.cu).  Plain torch: they run on the CPU, or in float64 on whatever device their inputs are on.
 
 Each precision recipe splits the two operands into planes with a fixed rounding -- power-of-two scales, fp16
 round-to-nearest high planes, fp16 or e4m3 correction planes -- and multiplies plane pairs on the tensor core, which forms
@@ -113,3 +114,144 @@ def prologue(x, a=None, b=None, act: str = "none", slope: float = 0.0) -> torch.
     elif act != "none":
         raise ValueError(act)
     return z
+
+
+# ------------------------------------------------------------------ GEMM and attention (linear_tc.cu, attention_tc.cu)
+# Both split every fp32 operand x into two fp16 planes, h = fp16(x) and l = fp16((x - h) * 2^11), and form a product as
+# h*h + (h*l + l*h) * 2^-11 (l*l, 2^-22 relative, is left out), with h*h and the correction in separate fp32 accumulators.
+LO_SCALE = 2048.0
+GEMM_KB = 32            # K block of one GEMM pipeline stage (linear_tc.cu KB)
+ATT_KB = 128            # key block of the attention kernel (attention_tc.cu KB)
+
+# Accumulation bounds, metric |y - y_ref| <= c * 2^-20 * scale per output element:
+#   GEMM       y_ref = linear(a, w, bias) (+ R), scale = sum_k |a_k||w_nk| + |bias_n| (+ |R|)       (sum_abs_linear)
+#   attention  y_ref = the float64 attention of the fp32 operands, scale = E of attention_bound
+# Measured on one H100 80GB HBM3 at a 400 W power limit over tests/test_gpu_linear_attention_tc.py: max 0.97 for the GEMM
+# (K = 2048, dense rows), 2.45 for the tensor-core attention (a peaked softmax over two key blocks: the tensor core
+# truncates each addition into the O accumulator, relative to the one dominant value), 0.80 for the SIMT attention.  The
+# weakest modelled defect scores 84 (GEMM) and 48 (attention) in the same metric (tests/test_cpu_gemm_attention_recipe.py).
+LINEAR_BOUND_C = 1.4
+ATTENTION_BOUND_C = 3.5
+ATTENTION_SIMT_BOUND_C = 1.2     # the fp32 SIMT attention kernel (rows.cu attention_kernel)     # the fp32 SIMT attention kernel (rows.cu), which st2_attention_ex runs
+
+
+def split2(x: torch.Tensor):
+    """fp32 x -> (h, l) as float64: h = fp16(x), l = fp16((x - h) * 2^11), as split2() of the GEMM and attention kernels.
+    x - h is exact in fp32, and so is the scaling by 2^11; fp16 rounding is round-to-nearest-even on both sides."""
+    x = x.float()
+    h = x.half()
+    return h.double(), ((x - h.float()) * LO_SCALE).half().double()
+
+
+def linear(a, w, bias=None, *, drop_hl_block=None, drop_lh_step=None) -> torch.Tensor:
+    """a [M,K] @ w[Nf,K]^T (+ bias) with the GEMM's operand planes, every plane product summed in float64.
+    Defects of a kernel, for the power test of the bound (tests/test_cpu_gemm_attention_recipe.py):
+      drop_hl_block = cb   the h(a)*l(w) product is lost on the 32-wide K block cb
+      drop_lh_step = s     the l(a)*h(w) product is lost on the 16-wide K step s"""
+    ah, al = split2(a)
+    wh, wl = split2(w)
+    hl, lh = ah @ wl.T, al @ wh.T
+    if drop_hl_block is not None:
+        k = slice(GEMM_KB * drop_hl_block, GEMM_KB * (drop_hl_block + 1))
+        hl = hl - ah[:, k] @ wl[:, k].T
+    if drop_lh_step is not None:
+        k = slice(16 * drop_lh_step, 16 * (drop_lh_step + 1))
+        lh = lh - al[:, k] @ wh[:, k].T
+    y = ah @ wh.T + (hl + lh) / LO_SCALE
+    return y if bias is None else y + bias.double()
+
+
+def sum_abs_linear(a, w, bias=None) -> torch.Tensor:
+    """sum_k |a_k||w_nk| (+ |bias_n|) of every output element: the scale of an fp32 dot product's rounding"""
+    s = a.double().abs() @ w.double().abs().T
+    return s if bias is None else s + bias.double().abs()
+
+
+def _valid_keys(lengths, B, N, device, extra=0):
+    klen = torch.full((B,), N, device=device) if lengths is None else lengths.to(device).long().clamp(max=N)
+    return torch.arange(N, device=device)[None, :] < (klen + extra).clamp(max=N)[:, None]          # [B, N]
+
+
+def attention_bound(q, k, v, lengths, scale, mutation=None, qchunk=64):
+    """q, k, v [B, N, H, 64] fp32; lengths [B] (keys n >= lengths[b] masked; clamped to N, as the kernels do) or None.
+    Returns (o, E), both [B, N, H, 64] float64:
+      o     softmax(scale q k^T) v in float64 (padded query rows included)
+      E     max_j(scale sum_e |q_ie||k_je|) * sum_j p_ij |v_jd - o_id|  +  sum_j p_ij |v_jd|   over valid keys j:
+            how an error in the logits propagates through the softmax, plus the two-plane rounding of P and V.
+    mutation: o is instead the kernel's two-plane recipe (operand planes of split2, P = exp(s - rowmax) split likewise,
+    sums in float64) with one defect, for the power test of the bound:
+      "recipe"             no defect (an accumulation-free kernel)
+      "p_low_last_block"   P's low plane is lost on the last key block
+      ("s_corr_step", i)   the correction products of S are lost on the 16-wide d step i
+      "mask_plus_one"      the mask admits one key too many (klen + 1)"""
+    B, N, H, Dh = q.shape
+    dev = q.device
+    qd, kd, vd = (t.double().permute(0, 2, 1, 3) for t in (q, k, v))               # [B, H, N, D]
+    valid = _valid_keys(lengths, B, N, dev)[:, None, None, :]                        # [B, 1, 1, N]
+    s = (qd @ kd.transpose(-1, -2)) * scale
+    p = torch.softmax(s.masked_fill(~valid, float("-inf")), -1)
+    o = p @ vd
+    smax = ((qd.abs() @ kd.abs().transpose(-1, -2)) * scale).masked_fill(~valid, 0).amax(-1, keepdim=True)
+    spread = torch.empty_like(o)
+    for i0 in range(0, N, qchunk):                                                    # sum_j p_ij |v_jd - o_id|
+        pi = p[:, :, i0:i0 + qchunk]
+        spread[:, :, i0:i0 + qchunk] = (pi[..., None] * (vd[:, :, None] - o[:, :, i0:i0 + qchunk, None]).abs()).sum(-2)
+    E = smax * spread + p @ vd.abs()
+    if mutation is not None:
+        o = _attention_recipe(q, k, v, lengths, scale, mutation)
+    return o.permute(0, 2, 1, 3), E.permute(0, 2, 1, 3)
+
+
+def _attention_recipe(q, k, v, lengths, scale, mutation):
+    B, N, H, Dh = q.shape
+    (qh, ql), (kh, kl), (vh, vl) = (tuple(x.permute(0, 2, 1, 3) for x in split2(t)) for t in (q, k, v))
+    corr_q, corr_k = ql.clone(), kl.clone()
+    if isinstance(mutation, tuple) and mutation[0] == "s_corr_step":
+        d = slice(16 * mutation[1], 16 * (mutation[1] + 1))
+        corr_q[..., d] = 0
+        corr_k[..., d] = 0
+    s = (qh @ kh.transpose(-1, -2) + (qh @ corr_k.transpose(-1, -2) + corr_q @ kh.transpose(-1, -2)) / LO_SCALE) * scale
+    valid = _valid_keys(lengths, B, N, q.device, 1 if mutation == "mask_plus_one" else 0)[:, None, None, :]
+    s = s.masked_fill(~valid, float("-inf"))
+    P = torch.exp(s - s.amax(-1, keepdim=True))
+    ph, pl = split2(P)
+    if mutation == "p_low_last_block":
+        nvalid = valid.sum(-1, keepdim=True)                                          # [B, 1, 1, 1]
+        last0 = (nvalid - 1) // ATT_KB * ATT_KB
+        pl = pl.masked_fill(torch.arange(N, device=q.device) >= last0, 0)
+    o = (ph @ vh + (ph @ vl + pl @ vh) / LO_SCALE) / P.sum(-1, keepdim=True)
+    return o
+
+
+def linear_operands(M, K, Nf, seed=0, *, bias=False, residual=False):
+    """Localised GEMM operands (a [M,K], w [Nf,K], bias [Nf] or None, R [M,Nf] or None; fp32): row m of a is non-zero only
+    on the 32-wide K block m mod ncb, except every 61st row, which is dense; |a| log-uniform over 1e-3 .. 1e2, random signs.
+    Every output element is then dominated by one K block (the tail block included), so a defect on one block or one
+    16-wide step shows at full size instead of diluted over all K."""
+    g = torch.Generator().manual_seed(seed)
+    ncb = (K + GEMM_KB - 1) // GEMM_KB
+    a = 10.0 ** (torch.rand(M, K, generator=g) * 5 - 3) * (torch.randint(0, 2, (M, K), generator=g) * 2 - 1)
+    rows = torch.arange(M)[:, None]
+    keep = (torch.arange(K)[None, :] // GEMM_KB == rows % ncb) | (rows % 61 == 7)
+    a = (a * keep).float()
+    w = torch.randn(Nf, K, generator=g) * 0.1
+    b = torch.randn(Nf, generator=g) * 0.1 if bias else None
+    r = torch.randn(M, Nf, generator=g) * 0.1 if residual else None
+    return a, w, b, r
+
+
+def attention_operands(B, N, H, lengths=None, seed=0, qscale=1.0):
+    """q, k, v [B, N, H, 64] fp32.  Keys and values are N(0, 1); query i of every head is qscale * (k_a + k_b) + N(0, 0.1)
+    for a random valid key a and a random key b of the utterance's LAST key block, so that (at scale 1/8) two keys carry
+    most of each row's softmax and the last block a large share of it: a defect there shows at full size."""
+    g = torch.Generator().manual_seed(seed)
+    k = torch.randn(B, N, H, 64, generator=g)
+    v = torch.randn(B, N, H, 64, generator=g)
+    klen = torch.full((B,), N) if lengths is None else lengths.long().clamp(max=N)
+    u1, u2 = torch.rand(B, N, H, generator=g), torch.rand(B, N, H, generator=g)
+    last0 = (klen - 1) // ATT_KB * ATT_KB
+    ia = (u1 * klen[:, None, None]).long()
+    ib = last0[:, None, None] + (u2 * (klen - last0)[:, None, None]).long()
+    take = lambda idx: torch.gather(k, 1, idx[..., None].expand(B, N, H, 64))     # noqa: E731
+    q = qscale * (take(ia) + take(ib)) + 0.1 * torch.randn(B, N, H, 64, generator=g)
+    return q.float(), k, v

@@ -17,7 +17,13 @@
 // recomputed in the second sweep: cheap, and O never needs rescaling); N <= 128 takes a single sweep.
 // Operands are staged into the K-major no-swizzle ("interleave") layout by the same threads: Q / K / P as
 // [k-chunk][row][8 x fp16], V transposed on the fly to [key-chunk][d][8 keys] (lanes run over d: coalesced global reads).
+// Range: the fp16 planes hold |q|, |k|, |v| < 65504; a larger (or NaN) staged value makes the output inf/NaN and raises a
+// range flag (as linear_tc.cu does), which st2_range_flag_fetch() reports and clears.  Masked keys and padded query rows
+// are staged as zeros and never raise it.  Every length must be >= 1: with no valid key the row sum is 0 and the output
+// non-finite (the SIMT kernel st2_attention_ex gives NaN there too).
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc_ptx.cuh"
@@ -42,6 +48,9 @@ constexpr int V_PLANE = (KB / 8) * V_LBO;                    // 16 KB
 constexpr int P_PLANE = (KB / 8) * Q_LBO;                    // 16 KB
 constexpr int SM_Q = 0, SM_K = SM_Q + 2 * Q_PLANE, SM_V = SM_K + 2 * K_PLANE, SM_P = SM_V + 2 * V_PLANE, SM_TOTAL = SM_P + 2 * P_PLANE;
 
+__device__ int g_range_flag = 0;
+constexpr float FP16_MAX = 65504.0f;
+
 struct Args {
   const float* q; long long q_ld;
   const float* k; const float* v; long long kv_ld;
@@ -58,9 +67,15 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& p0, uint32_
   p0 = *reinterpret_cast<const uint32_t*>(&h);
   p1 = *reinterpret_cast<const uint32_t*>(&l);
 }
-// 8 fp32 -> one 16-byte row of each plane
-__device__ __forceinline__ void store_row8(uint8_t* plane0, int plane_bytes, size_t off, const float (&x)[8]) {
+// 8 fp32 -> one 16-byte row of each plane; with CHECK, in_range stays true while every value fits the fp16 planes (false
+// for NaN)
+template <bool CHECK = true>
+__device__ __forceinline__ void store_row8(uint8_t* plane0, int plane_bytes, size_t off, const float (&x)[8], bool& in_range) {
   uint32_t a[4], b[4];
+  if (CHECK) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) in_range &= fabsf(x[i]) < FP16_MAX;
+  }
 #pragma unroll
   for (int i = 0; i < 4; ++i) split2(x[2 * i], x[2 * i + 1], a[i], b[i]);
   *reinterpret_cast<uint4*>(plane0 + off) = make_uint4(a[0], a[1], a[2], a[3]);
@@ -80,6 +95,7 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
   const int klen = a.lengths ? min(a.lengths[b], N) : N;
   const int nkb = max(1, (klen + KB - 1) / KB);
   const long long rowbase = (long long)b * N;
+  bool in_range = true;
 
   // ---- stage Q (once): thread t -> query row t % 64, four 8-wide chunks of d
   {
@@ -93,10 +109,12 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = 0.f;
       }
-      store_row8(smem + SM_Q, Q_PLANE, (size_t)c * Q_LBO + (size_t)r * ROWS16, x);
+      store_row8(smem + SM_Q, Q_PLANE, (size_t)c * Q_LBO + (size_t)r * ROWS16, x, in_range);
     }
   }
-  auto stage_k = [&](int kb) {      // thread t -> key kb*128 + t
+  // thread t -> key kb*128 + t.  check = std::true_type range-checks the keys; sweep 1 stages the same keys as sweep 2 and
+  // passes std::false_type
+  auto stage_k = [&](int kb, auto check) {
     const int key = kb * KB + tid;
     const float* kr = a.k + (rowbase + min(key, N - 1)) * a.kv_ld + h * HD;
 #pragma unroll
@@ -107,7 +125,7 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = 0.f;
       }
-      store_row8(smem + SM_K, K_PLANE, (size_t)c * K_LBO + (size_t)tid * ROWS16, x);
+      store_row8<decltype(check)::value>(smem + SM_K, K_PLANE, (size_t)c * K_LBO + (size_t)tid * ROWS16, x, in_range);
     }
   };
   auto stage_v = [&](int kb) {      // thread t -> d = t % 64, key chunks (t / 64) * 8 .. + 7; V^T rows of 8 keys
@@ -120,7 +138,7 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
         const int key = kb * KB + c * 8 + i;
         x[i] = key < klen ? __ldg(a.v + (rowbase + key) * a.kv_ld + h * HD + d) : 0.f;
       }
-      store_row8(smem + SM_V, V_PLANE, (size_t)c * V_LBO + (size_t)d * ROWS16, x);
+      store_row8(smem + SM_V, V_PLANE, (size_t)c * V_LBO + (size_t)d * ROWS16, x, in_range);
     }
   };
   float sm[64], sc[64];             // S fragment: row 16 w + g + 8 i, key 8 j + 2 t4 + c  ->  index 4 j + 2 i + c
@@ -181,7 +199,7 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
   // ---- sweep 1 (only when there are several key blocks): row maxima
   if (two_pass) {
     for (int kb = 0; kb < nkb; ++kb) {
-      stage_k(kb);
+      stage_k(kb, std::false_type{});
       fence_proxy_async();
       __syncthreads();
       compute_s();
@@ -191,7 +209,7 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
   }
   // ---- sweep 2: P and O
   for (int kb = 0; kb < nkb; ++kb) {
-    stage_k(kb);
+    stage_k(kb, std::true_type{});
     stage_v(kb);
     fence_proxy_async();
     __syncthreads();
@@ -236,9 +254,19 @@ __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) 
       if (row < N) *reinterpret_cast<float2*>(orow + 8 * j + 2 * t4) = o;
     }
   }
+  if (!in_range) atomicExch(&g_range_flag, 1);
 }
 
 }  // namespace atc
+
+cudaError_t attention_tc_range_flag_fetch(int* flag) {
+  int v = 0, zero = 0;
+  cudaError_t e = cudaMemcpyFromSymbol(&v, atc::g_range_flag, sizeof(int));   // synchronises with the device
+  if (e == cudaSuccess && v) e = cudaMemcpyToSymbol(atc::g_range_flag, &zero, sizeof(int));
+  *flag = v;
+  return e;
+}
+
 }  // namespace st2
 
 using namespace st2;

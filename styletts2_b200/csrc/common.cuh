@@ -15,6 +15,8 @@ void set_error_msg(const char* where, const char* msg);
 
 // Range flag of the tensor-core convs (conv_tc.cu): reads and clears it; st2_range_flag_fetch reports it with the GEMMs' flag.
 cudaError_t conv_tc_range_flag_fetch(int* flag);
+// The same for the tensor-core attention (attention_tc.cu).
+cudaError_t attention_tc_range_flag_fetch(int* flag);
 
 #define ST2_CHECK_LAUNCH(where)                         \
   do {                                                  \

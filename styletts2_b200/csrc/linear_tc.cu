@@ -56,12 +56,15 @@ constexpr int B_WFULL = 0, B_WEMPTY = 6, B_AFULL = 12, B_AEMPTY = 16, B_COUNT = 
 using namespace st2::ptx;
 
 // Range guard: the fp16 planes hold |x| < 65504; larger activations become inf (and the product NaN/inf).  Every thread
-// that splits activations tracks its own maximum and raises this flag once; st2_range_flag_fetch() reports and clears
-// it (the host checks it after a pass, styletts2_b200.ops.check_range).  Weights are checked when they are laid out.
+// that splits activations keeps one predicate over the values it converts and raises this flag once;
+// st2_range_flag_fetch() reports and clears it (the host checks it after a pass, styletts2_b200.ops.check_range).
+// Weights are checked when they are laid out.  The predicate is an AND of fabsf(x) < FP16_MAX, which is false for NaN
+// (a running fmaxf maximum is not: fmaxf drops a NaN argument).
 __device__ int g_range_flag = 0;
 constexpr float FP16_MAX = 65504.0f;
-__device__ __forceinline__ void range_note(float amax) {
-  if (!(amax < FP16_MAX)) atomicExch(&g_range_flag, 1);   // also catches NaN
+__device__ __forceinline__ bool in_fp16_range(float x) { return fabsf(x) < FP16_MAX; }
+__device__ __forceinline__ void range_note(bool in_range) {
+  if (!in_range) atomicExch(&g_range_flag, 1);
 }
 
 // x0,x1 -> two packed fp16 pairs: p0 = fp16(x), p1 = fp16((x - p0) * 2^11)   (x = p0 + p1 * 2^-11 to ~2^-22 |x|)
@@ -225,10 +228,11 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
         }
       };
       load_blk(0, cur);
-      float amax = 0.f;
+      bool in_range = true;
       for (int cb = 0; cb < ncb; ++cb) {
 #pragma unroll
-        for (int q = 0; q < 2; ++q) amax = fmaxf(amax, fmaxf(fmaxf(fabsf(cur[q].x), fabsf(cur[q].y)), fmaxf(fabsf(cur[q].z), fabsf(cur[q].w))));
+        for (int q = 0; q < 2; ++q)
+          in_range &= in_fp16_range(cur[q].x) & in_fp16_range(cur[q].y) & in_fp16_range(cur[q].z) & in_fp16_range(cur[q].w);
         if (cb + 1 < ncb) load_blk(cb + 1, nxt);
         mbar_wait(BAR(B_AEMPTY + as), aph ^ 1);
         uint8_t* base = smem + SM_A + as * A_BUF_BYTES;
@@ -246,7 +250,7 @@ __global__ void __launch_bounds__(THREADS, 1) linear_tc_kernel(const LinArgs a, 
 #pragma unroll
         for (int q = 0; q < 2; ++q) cur[q] = nxt[q];
       }
-      range_note(amax);
+      range_note(in_range);
     }
   }
 }
@@ -278,10 +282,10 @@ __global__ void linear_tc_split_kernel(const float* __restrict__ A, long long ld
           if (k0 + j < K) x[j] = __ldg(p + j);
       }
     }
-    float amax = 0.f;
+    bool in_range = true;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) amax = fmaxf(amax, fabsf(x[j]));
-    range_note(amax);
+    for (int j = 0; j < 8; ++j) in_range &= in_fp16_range(x[j]);
+    range_note(in_range);
     uint32_t p0[4], p1[4];
 #pragma unroll
     for (int q = 0; q < 4; ++q) split2(x[2 * q], x[2 * q + 1], p0[q], p1[q]);
@@ -307,7 +311,7 @@ __global__ void linear_tc_weight_layout_kernel(const float* __restrict__ w, __ha
     const int n = cob * TMF + col, k = cb * KB + kc * 8 + j;
     float v = 0.f;
     if (n < Nf && k < K) v = w[(long long)n * K + k];
-    range_note(fabsf(v));
+    range_note(in_fp16_range(v));
     const __half h0 = __float2half_rn(v);
     const __half h1 = __float2half_rn((v - __half2float(h0)) * LO_SCALE);
     out[i] = pl == 0 ? h0 : h1;
@@ -326,10 +330,11 @@ int st2_range_flag_fetch(int* flag_out) {
   int v = 0, zero = 0;
   cudaError_t e = cudaMemcpyFromSymbol(&v, ltc::g_range_flag, sizeof(int));     // synchronises with the device
   if (e == cudaSuccess && v) e = cudaMemcpyToSymbol(ltc::g_range_flag, &zero, sizeof(int));
-  int vc = 0;
+  int vc = 0, va = 0;
   if (e == cudaSuccess) e = conv_tc_range_flag_fetch(&vc);                       // the tensor-core convs' flag (conv_tc.cu)
+  if (e == cudaSuccess) e = attention_tc_range_flag_fetch(&va);                  // the tensor-core attention's (attention_tc.cu)
   if (e != cudaSuccess) { set_error("st2_range_flag_fetch", e); return (int)e; }
-  *flag_out = v | vc;
+  *flag_out = v | vc | va;
   return 0;
 }
 

@@ -392,15 +392,16 @@ def linear(A, W, bias=None, *, act=ACT_NONE, R=None, out=None, wtc=None):
 
 
 def check_range():
-    """Raise if any fp16-plane operand of a tensor-core GEMM or conv since the last check left fp16's range or was NaN
-    (GEMM: |x| >= 65504; conv, after its power-of-two operand scales: |z| >= 65504/64 after the prologue, |w| >= 65504/4096):
-    the outputs of that pass hold inf/NaN.  Clears the flag.  Synchronises; not callable under CUDA-graph capture."""
+    """Raise if any fp16-plane operand of a tensor-core GEMM, attention or conv since the last check left fp16's range or
+    was NaN (GEMM and attention: |x| >= 65504 for the activations, weights, q, k and v; conv, after its power-of-two operand
+    scales: |z| >= 65504/64 after the prologue, |w| >= 65504/4096): the outputs of that pass hold inf/NaN.  Clears the
+    flag.  Synchronises; not callable under CUDA-graph capture."""
     flag = C.c_int(0)
     L.call("st2_range_flag_fetch", C.byref(flag))
     if flag.value:
-        raise FloatingPointError("styletts2_b200: an operand of a tensor-core GEMM or conv exceeded the fp16 plane range "
-                                 "(GEMM |x| >= 65504; conv |activation| >= 1023.5 or |weight| >= 16) or was NaN; set ST2_TC=0 "
-                                 "to run these layers on the fp32 SIMT kernels")
+        raise FloatingPointError("styletts2_b200: an operand of a tensor-core GEMM, attention or conv exceeded the fp16 plane "
+                                 "range (GEMM / attention |x| >= 65504; conv |activation| >= 1023.5 or |weight| >= 16) or was "
+                                 "NaN; set ST2_TC=0 to run these layers on the fp32 SIMT kernels")
 
 
 def linear_strided(x, B, Lr, K, bs, ls, ks, W, bias=None, *, act=ACT_NONE, out=None):
