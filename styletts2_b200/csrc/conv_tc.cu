@@ -1,6 +1,6 @@
 // Tensor-core (wgmma) implicit-GEMM Conv1d for the vocoder's AdaIN ResBlocks -- sm_90a.
 //
-//   D[co (M=128), t (N=64)] = sum_{tap} sum_{ci} W_tap[co, ci] * z[ci, t + tap*dil - pad],   z = snake/lrelu(a*x+b)
+//   D[co (M=128), t (N=128)] = sum_{tap} sum_{ci} W_tap[co, ci] * z[ci, t + tap*dil - pad],   z = snake/lrelu(a*x+b)
 //
 // Precision recipes (decided with the CPU oracle by emulation, DESIGN.md "precision"; tools/emulate_precision.py):
 // operands are pre-scaled by exact powers of two, w' = w * 2^12 and z' = z * 2^6 (the epilogue multiplies by 2^-18), so
@@ -21,18 +21,20 @@
 //  * A operand = weights  [64 co x 16 ci] per consumer warpgroup, K-major, no-swizzle "interleave" layout (8-row x 16-byte
 //    core matrices, rows contiguous at 16 B pitch).  Pre-arranged in HBM so that one pipeline stage (taps, 16 ci, both
 //    planes) is ONE contiguous block moved by a single 1-D TMA bulk copy (cp.async.bulk) that signals an mbarrier.
-//  * B operand = activations [64 t x 16 ci], K-major, same interleave layout: for each K chunk the frame window is a
+//  * B operand = activations [128 t x 16 ci], K-major, same interleave layout: for each K chunk the frame window is a
 //    column of 16-byte rows, so a conv tap is just a descriptor start address shifted by tap*dil rows (16 B
 //    granularity) -- the window is staged ONCE per 16-channel block (AdaIN affine + Snake/LeakyReLU + plane split
 //    fused into the staging) and re-used by all K taps.
 //  * Raw fp32 frame windows travel HBM -> shared memory as 16-byte cp.async copies of the ALIGNED superset window of
 //    every channel row (rows of odd length start at any 4-byte phase; the phase becomes a per-channel offset of the
 //    scalar shared-memory reads of the conversion), four blocks in flight per SM.
-//  * D accumulators live in the registers of two consumer warpgroups (output channels 0-63 / 64-127 of the tile); the
-//    epilogue works on the fragments and fuses bias, residual, MRF accumulation and the InstanceNorm partial statistics
-//    (count, mean, M2 per 64-frame tile) exactly like the SIMT kernel.
-//  * Warp roles: warps 0-7 = consumers (wgmma + epilogue), warp 8 = weight TMA producer, warps 9-18 = activation stagers.
-//    Persistent CTAs (one per SM) loop over tiles.
+//  * D accumulators live in the registers of two consumer warpgroups (output channels 0-63 / 64-127 of the tile, 128 frames
+//    each: m64n128 MMAs); the epilogue works on the fragments and fuses bias, residual, MRF accumulation and the InstanceNorm
+//    partial statistics (count, mean, M2) exactly like the SIMT kernel.  A 128-frame tile writes two partials, one per
+//    64 frames, so the statistics layout does not depend on the tile width.
+//  * Warp roles in whole warpgroups: warps 0-7 = consumers (wgmma + epilogue), warp 8 = weight TMA producer, warps 9-14 =
+//    activation stagers, warp 15 idle.  setmaxnreg moves registers from warpgroups 2-3 to the consumers (arithmetic at
+//    THREADS below).  Persistent CTAs (one per SM) loop over tiles.
 //
 // TWO kernels share the stager and weight-producer roles (device functions below): the channel-major conv1d_tc_kernel
 // described above and the TIME-MAJOR conv1d_tct_kernel further down (FAST recipe, Cout <= 128: frames on the MMA's M axis,
@@ -50,8 +52,9 @@ namespace tc {
 
 constexpr int MODE_FAST = ST2_TC_FAST, MODE_ACC = ST2_TC_ACCURATE, MODE_X3 = ST2_TC_F16X3;
 
-constexpr int TN = 64;                          // frames per tile (wgmma N of the channel-major kernel, M of the time-major one)
-constexpr int TM = 128;                         // output channels per tile of the channel-major kernel (two warpgroups of M = 64)
+constexpr int TN = 128;                         // frames per tile (wgmma N of the channel-major kernel; 2 x M = 64 of the time-major one)
+constexpr int TP = 64;                          // frames per InstanceNorm statistics partial: a tile writes TN / TP of them
+constexpr int TM = 128;                        // output channels per tile of the channel-major kernel (two warpgroups of M = 64)
 constexpr int CB = 16;                          // input channels per pipeline block (one UMMA K step of the fp16 planes)
 constexpr int KCB = CB / 8;                     // 16-byte K chunks per plane and block
 constexpr int W_PLANE_BYTES = KCB * TM * 16;    // 4 KB
@@ -61,24 +64,35 @@ constexpr int TPS = 2;                          // taps per pipeline stage: one 
                                                 // as the 2 MMAs of one tap)
 constexpr int W_STAGE_BYTES = TPS * W_STEP_BYTES;  // 16 KB
 constexpr int W_STAGES = 3;                     // 48 KB (6 taps) of weights in flight per SM
-constexpr int RW_MAX = 312;                     // TN + (K-1)*dil rounded up to 8, max
+constexpr int RW_MAX = 312;                     // TN + (K-1)*dil rounded up to 8, max: (K-1)*dil <= 184 (the models need <= 50)
 constexpr int RWP_MAX = RW_MAX + 2;             // chunk pitch in rows of the staged planes
 constexpr int ACT_PLANE_BYTES = KCB * RWP_MAX * 16;  // one plane of one 16-channel block
 constexpr int ACT_BUF_BYTES = 2 * ACT_PLANE_BYTES;
-constexpr int RAW_STAGES = 4;                   // cp.async ring of raw fp32 frame windows: 3 blocks (60 KB) in flight per SM
-constexpr int RAW_CHUNKS = 80;                  // 16-byte chunks copied per channel row: 320 floats >= RW_MAX + 3
-constexpr int RAW_PITCH = 336;                  // floats per channel row of a raw block: pitch = 64 bytes mod 128, so that the 32 cp.async
-                                                // destinations of a warp (20 chunks of one row, 12 of the next) fall on distinct banks
-                                                // (ncu: 3x excess shared-memory wavefronts of the LDGSTS at a pitch of 1280 bytes; the
-                                                // shared-memory data pipe is shared with the tensor core's operand reads)
-constexpr int RAW_BYTES = CB * RAW_PITCH * 4;   // 20 KB
+constexpr int RAW_STAGES = 4;                   // cp.async ring of raw fp32 frame windows: 3 blocks (63 KB) in flight per SM
+constexpr int RAW_CHUNKS = 84;                  // 16-byte chunks copied per channel row: 336 floats >= RW_MAX + 3
+constexpr int RAW_PITCH = 336;                  // floats per channel row of a raw block: pitch = 64 bytes mod 128.  The 32 cp.async
+                                                // destinations of a warp cover chunk runs of 12 (one row each) at row offsets that
+                                                // alternate between 0 and 64 bytes mod 128, which puts exactly 4 of them on every
+                                                // 16-byte bank group (ncu, earlier layout: 3x excess shared-memory wavefronts of the
+                                                // LDGSTS at a pitch of 1280 bytes; the shared-memory data pipe is shared with the
+                                                // tensor core's operand reads)
+constexpr int RAW_BYTES = CB * RAW_PITCH * 4;   // 21 KB
 constexpr int CIN_PAD_MAX = 1120;
-constexpr int NUM_STAGERS = 320;                // 10 warps (8 would not buy registers: allocation is per 4 warps, 18 -> 20)
+// Warp roles in whole warpgroups, so that each can set its own register budget (setmaxnreg):
+//   warpgroups 0-1 (warps 0-7): consumers, 64 frames x Cout (time-major) or 64 channels x 128 frames (channel-major) each
+//   warp 8: weight TMA producer; warps 9-14: activation stagers; warp 15: idle
+// The launch allocates 512 threads x 128 registers = 64 K, the whole register file.  The producer warpgroups give
+// 2 x 128 x (128 - 64) registers back, which the consumers take: 2 x 128 x 192 + 2 x 128 x 64 = 65536.  A consumer holds two
+// 64-register fp32 accumulators (FAST / ACCURATE; 64 x 128 per warpgroup).
+constexpr int NUM_CONS = 256;                   // two consumer warpgroups
+constexpr int NUM_STAGERS = 192;                // 6 warps: an even count (the conversion mapping pairs warps over the K chunks)
 constexpr int ST_PER_CH = NUM_STAGERS / CB;     // issue mapping: threads per channel row of a raw block
 constexpr int ROWS_PER_PASS = (NUM_STAGERS / 64) * 32;  // conversion mapping: rows covered per pass
-constexpr int NUM_CONS = 256;                   // two consumer warpgroups
 constexpr int ST0 = NUM_CONS + 32;              // first stager thread (warp 8 is the weight producer)
-constexpr int THREADS = ST0 + NUM_STAGERS;      // 608 = 19 warps
+constexpr int THREADS = 512;                    // 4 warpgroups
+constexpr int REG_LAUNCH = 128, REG_CONS = 192, REG_AUX = 64;
+static_assert(ST0 + NUM_STAGERS <= THREADS && THREADS * REG_LAUNCH <= 65536, "thread roles");
+static_assert(NUM_CONS * REG_CONS + (THREADS - NUM_CONS) * REG_AUX <= THREADS * REG_LAUNCH, "register budget");
 
 // power-of-two operand scaling (exact): w' = w * 2^12, z' = z * 2^6; accumulators hold 2^18 x the convolution
 constexpr float W_SCALE = 4096.0f, X_SCALE = 64.0f, D_UNSCALE = 1.0f / (4096.0f * 64.0f);
@@ -98,9 +112,11 @@ constexpr int SM_ACT = SM_W + W_STAGES * W_STAGE_BYTES;
 constexpr int SM_RAW = SM_ACT + 2 * ACT_BUF_BYTES;
 constexpr int SM_COEF = SM_RAW + RAW_STAGES * RAW_BYTES;
 constexpr int SM_EPI = SM_COEF + 4 * CIN_PAD_MAX * 4;   // per-channel prologue coefficients of the current utterance (4 x 1120 floats)
-constexpr int SM_BAR = SM_EPI + 2 * 4 * 64 * 4;   // time-major statistics scratch [2 warpgroups][4 warps][64 channels]
+constexpr int TCT_NC_MAX = 128;                   // output channels of the time-major kernel, max
+constexpr int SM_BAR = SM_EPI + 2 * 4 * TCT_NC_MAX * 4;   // time-major statistics scratch [2 warpgroups][4 warps][128 channels]
 constexpr int SM_TOTAL = SM_BAR + 512;
-static_assert(RAW_CHUNKS % ST_PER_CH == 0 && NUM_STAGERS % 64 == 0, "stager mappings");
+static_assert(RAW_CHUNKS % ST_PER_CH == 0 && NUM_STAGERS % 64 == 0 && NUM_STAGERS % CB == 0, "stager mappings");
+static_assert(RAW_CHUNKS * 4 >= RW_MAX + 3 && RAW_PITCH >= RAW_CHUNKS * 4 && (RAW_PITCH * 4) % 128 == 64, "raw window rows");
 static_assert(SM_TOTAL <= 232448, "shared memory budget (227 KB per CTA)");
 
 // barrier slots (8 B each) inside SM_BAR
@@ -235,7 +251,7 @@ __device__ __forceinline__ void stager_role(const st2_conv_args& a, uint8_t* sme
   // copies the 16-byte ALIGNED superset of its window; the phase (0..3 floats) is re-derived by the conversion.
   // Chunks outside the tensor are zero-filled (src-size 0), the chunk that crosses the end of the tensor is
   // trimmed; nothing before the 16-byte aligned start of the tensor's allocation is ever touched.
-  const int st = tid - ST0;  // 0..319
+  const int st = tid - ST0;  // 0..NUM_STAGERS-1
   const int Lin_ = a.Lin, pre_act_ = a.pre_act, Cin_ = a.Cin;
   const float slope_ = a.pre_slope;
   const bool has_affine = a.pre_a != nullptr, is_snake = pre_act_ == ST2_ACT_SNAKE;
@@ -393,15 +409,33 @@ __device__ __forceinline__ void release(const uint32_t bar0, const Pending& p, c
   }
 }
 
-// Output value of one element: bias, residual, divisor, MRF accumulation into y and output activation, in the order of the
-// SIMT kernel.  Returns the value written (the InstanceNorm statistics are taken of it).
-__device__ __forceinline__ float epi_value(const st2_conv_args& a, float v, float bias, const float* rrow, float* yp, int oidx) {
+// Output value of one element: bias, residual, divisor, MRF accumulation and output activation, in the order of the SIMT
+// kernel.  res_v = the residual, y_old = the y value the MRF accumulation adds to (each read only when its mode is on).
+__device__ __forceinline__ float epi_combine(const st2_conv_args& a, float v, float bias, float res_v, float y_old) {
   float val = v + bias;
-  if (rrow) val += rrow[oidx >> a.res_shift];
+  if (a.res) val += res_v;
   if (a.out_div != 1.0f) val = __fdiv_rn(val, a.out_div);
-  if (a.accum_mode == 1) val = yp[oidx] + val;
-  else if (a.accum_mode == 2) val = __fdiv_rn(yp[oidx] + val, a.accum_div);
+  if (a.accum_mode == 1) val = y_old + val;
+  else if (a.accum_mode == 2) val = __fdiv_rn(y_old + val, a.accum_div);
   if (a.out_act == ST2_ACT_TANH) val = tanhf(val);
+  return val;
+}
+
+// The epilogues read the residual and MRF operands of a group of elements BEFORE they store any of them.  The compiler
+// may not move a load above a store through a pointer that could alias it, so loading each element's operands just before
+// its store pays one full memory latency per element (the consumer warps have nothing else to issue meanwhile).  An
+// element's operands are only ever read by the thread that writes it, so the values are the same.
+__device__ __forceinline__ void epi_load(const st2_conv_args& a, const float* rrow, const float* yp, int oidx, bool ok, float& res_v,
+                                         float& y_old) {
+  res_v = (rrow && ok) ? rrow[oidx >> a.res_shift] : 0.f;
+  y_old = (a.accum_mode != 0 && ok) ? yp[oidx] : 0.f;
+}
+
+// One element, loads and store together (the reflection duplicate, one element per row).  Returns the value written.
+__device__ __forceinline__ float epi_value(const st2_conv_args& a, float v, float bias, const float* rrow, float* yp, int oidx) {
+  float res_v, y_old;
+  epi_load(a, rrow, yp, oidx, true, res_v, y_old);
+  const float val = epi_combine(a, v, bias, res_v, y_old);
   yp[oidx] = val;
   return val;
 }
@@ -431,6 +465,7 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
 
   if (warp < NUM_CONS / 32) {
     // ================================================================ consumers: wgmma (warpgroup wg = channels 64 wg ..) + epilogue
+    reg_alloc<REG_CONS>();
     const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
     const bool leader = (tid & 127) == 0;
     const uint32_t lbo_a = TM * 16, lbo_b = (uint32_t)RWP * 16;
@@ -439,9 +474,9 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
     Pending pend{-1, -1};
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const TileCoord tc_ = tile_coord(tile, n_tq, n_cob);
-      float d0[32], d1[32];
+      float d0[64], d1[64];
 #pragma unroll
-      for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+      for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
       uint32_t acc = 0;
       for (int cb = 0; cb < ncb; ++cb) {
         mbar_wait(BAR(B_AFULL + as), aph);
@@ -457,16 +492,16 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
               const uint64_t da0 = make_desc(a_addr, lbo_a, 128), da1 = make_desc(a_addr + W_PLANE_BYTES, lbo_a, 128);
               const uint64_t db0 = make_desc(b_addr, lbo_b, 128), db1 = make_desc(b_addr + ACT_PLANE_BYTES, lbo_b, 128);
               if (MODE == MODE_FAST) {
-                wgmma_f16_n64(d0, da0, db0, acc);
-                wgmma_e4m3_n64(d1, da1, db1, acc);     // both corrections in one e4m3 K=32 MMA, own accumulator
+                wgmma_f16_n128(d0, da0, db0, acc);
+                wgmma_e4m3_n128(d1, da1, db1, acc);     // both corrections in one e4m3 K=32 MMA, own accumulator
               } else if (MODE == MODE_ACC) {
-                wgmma_f16_n64(d0, da0, db0, acc);
-                wgmma_f16_n64(d1, da0, db1, acc);
-                wgmma_f16_n64(d1, da1, db0, 1u);
+                wgmma_f16_n128(d0, da0, db0, acc);
+                wgmma_f16_n128(d1, da0, db1, acc);
+                wgmma_f16_n128(d1, da1, db0, 1u);
               } else {
-                wgmma_f16_n64(d0, da0, db0, acc);
-                wgmma_f16_n64(d0, da0, db1, 1u);
-                wgmma_f16_n64(d0, da1, db0, 1u);
+                wgmma_f16_n128(d0, da0, db0, acc);
+                wgmma_f16_n128(d0, da0, db1, 1u);
+                wgmma_f16_n128(d0, da1, db0, 1u);
               }
               acc = 1;
               a_addr += W_STEP_BYTES;
@@ -487,113 +522,147 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
       if (MODE != MODE_X3) wg_fence_regs(d1);
       release(bar0, pend, leader);
       pend.ws = -1;
+      // fold the correction accumulator: d0 holds the unscaled sums from here on (d1 is dead)
+#pragma unroll
+      for (int r = 0; r < 64; ++r) {
+        float v = d0[r];
+        if (MODE == MODE_ACC) v = fmaf(d1[r], ACC_LO_UNSCALE, v);
+        if (MODE == MODE_FAST) v += d1[r];
+        d0[r] = v * D_UNSCALE;
+      }
 
-      // ---- epilogue: row = output channel, column = frame
-      const int t0 = tc_.tq * TN;
-      const int ncols = min(TN, a.Lq - t0);
+      // ---- epilogue: row = output channel, column = frame; each 64-frame half of the tile (fragment columns j = 8 h ..
+      // 8 h + 7) is one statistics partial.  The second half of a tail tile can lie entirely beyond Lq: no partial then.
       float* yb = a.y + (long long)tc_.b * a.y_bstride;
       const float* rbase = a.res ? a.res + (long long)tc_.b * a.res_bstride : nullptr;
+      float biases[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
+        biases[i] = (a.bias && co < a.Cout) ? a.bias[co] : 0.f;
+      }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
         const bool cok = co < a.Cout;
-        const float bias = (a.bias && cok) ? a.bias[co] : 0.f;
+        const float bias = biases[i];
         float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
         const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
-        float vals[16];
-        float s = 0.f, n = 0.f;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int h = 0; h < TN / TP; ++h) {
+          const int t0 = tc_.tq * TN + h * TP;
+          const int ncols = min(TP, a.Lq - t0);
+          float s = 0.f, n = 0.f;
 #pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int r = 4 * j + 2 * i + c, col = 8 * j + 2 * t4 + c;
-            float v = d0[r];
-            if (MODE == MODE_ACC) v = fmaf(d1[r], ACC_LO_UNSCALE, v);
-            if (MODE == MODE_FAST) v += d1[r];
-            v *= D_UNSCALE;
-            float val = 0.f;
-            if (cok && col < ncols) {
-              val = epi_value(a, v, bias, rrow, yp, (t0 + col) * a.y_tstride + a.y_toffset);
-              s += val;
-              n += 1.f;
+          for (int j0 = 0; j0 < 8; j0 += 4) {
+            float res_v[8], y_old[8];   // 8 elements of this row: operands first, then the stores (epi_load)
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+#pragma unroll
+              for (int c = 0; c < 2; ++c) {
+                const int col = 8 * (j0 + jj) + 2 * t4 + c;
+                epi_load(a, rrow, yp, (t0 + col) * a.y_tstride + a.y_toffset, cok && col < ncols, res_v[2 * jj + c], y_old[2 * jj + c]);
+              }
             }
-            vals[2 * j + c] = val;
-            // ReflectionPad1d((1,0)) duplicate of the q==0 column (istftnet.py:365-366): value differs by its residual
-            if (col == 0 && t0 == 0 && a.dup_q0_to >= 0 && cok) {
-              const float dv = epi_value(a, v, bias, rrow, yp, a.dup_q0_to);
-              s += dv;   // one extra sample of this row
-              n += 1.f;
-            }
-          }
-        }
-        if (a.stats) {
-          // two-pass (count, mean, M2) of the row over the tile's frames: the four lanes t4 of a quad share the row
-          s += __shfl_xor_sync(0xffffffffu, s, 1);
-          s += __shfl_xor_sync(0xffffffffu, s, 2);
-          n += __shfl_xor_sync(0xffffffffu, n, 1);
-          n += __shfl_xor_sync(0xffffffffu, n, 2);
-          const float mean = n > 0.f ? s / n : 0.f;
-          float m2 = 0.f;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
+            for (int jj = 0; jj < 4; ++jj) {
 #pragma unroll
-            for (int c = 0; c < 2; ++c) {
-              const int col = 8 * j + 2 * t4 + c;
-              const float dv = vals[2 * j + c] - mean;
-              if (col < ncols) m2 = fmaf(dv, dv, m2);
+              for (int c = 0; c < 2; ++c) {
+                const int j = j0 + jj;
+                const int r = 4 * (8 * h + j) + 2 * i + c, col = 8 * j + 2 * t4 + c;
+                const float v = d0[r];
+                float val = 0.f;
+                if (cok && col < ncols) {
+                  val = epi_combine(a, v, bias, res_v[2 * jj + c], y_old[2 * jj + c]);
+                  yp[(t0 + col) * a.y_tstride + a.y_toffset] = val;
+                  s += val;
+                  n += 1.f;
+                }
+                d0[r] = val;
+                // ReflectionPad1d((1,0)) duplicate of the q==0 column (istftnet.py:365-366): value differs by its residual
+                if (col == 0 && t0 == 0 && a.dup_q0_to >= 0 && cok) {
+                  const float dv = epi_value(a, v, bias, rrow, yp, a.dup_q0_to);
+                  s += dv;   // one extra sample of this row
+                  n += 1.f;
+                }
+              }
             }
           }
-          if (t0 == 0 && a.dup_q0_to >= 0 && t4 == 0 && cok) {
-            const float dv = yp[a.dup_q0_to] - mean;
-            m2 = fmaf(dv, dv, m2);
-          }
-          m2 += __shfl_xor_sync(0xffffffffu, m2, 1);
-          m2 += __shfl_xor_sync(0xffffffffu, m2, 2);
-          if (t4 == 0 && cok) {
-            float* sp = a.stats + (((long long)tc_.b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + tc_.tq) * 3;
-            sp[0] = n; sp[1] = mean; sp[2] = m2;
+          if (a.stats && ncols > 0) {
+            // two-pass (count, mean, M2) of the row over the half's frames: the four lanes t4 of a quad share the row
+            s += __shfl_xor_sync(0xffffffffu, s, 1);
+            s += __shfl_xor_sync(0xffffffffu, s, 2);
+            n += __shfl_xor_sync(0xffffffffu, n, 1);
+            n += __shfl_xor_sync(0xffffffffu, n, 2);
+            const float mean = n > 0.f ? s / n : 0.f;
+            float m2 = 0.f;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+              for (int c = 0; c < 2; ++c) {
+                const int col = 8 * j + 2 * t4 + c;
+                const float dv = d0[4 * (8 * h + j) + 2 * i + c] - mean;
+                if (col < ncols) m2 = fmaf(dv, dv, m2);
+              }
+            }
+            if (t0 == 0 && a.dup_q0_to >= 0 && t4 == 0 && cok) {
+              const float dv = yp[a.dup_q0_to] - mean;
+              m2 = fmaf(dv, dv, m2);
+            }
+            m2 += __shfl_xor_sync(0xffffffffu, m2, 1);
+            m2 += __shfl_xor_sync(0xffffffffu, m2, 2);
+            if (t4 == 0 && cok) {
+              const int part = tc_.tq * (TN / TP) + h;
+              float* sp = a.stats + (((long long)tc_.b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + part) * 3;
+              sp[0] = n; sp[1] = mean; sp[2] = m2;
+            }
           }
         }
       }
     }
-  } else if (warp == NUM_CONS / 32) {
-    // ================================================================ weight producer (1-D TMA bulk copies)
-    if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, W_STEP_BYTES, TPS, W_STAGE_BYTES, ntiles, n_tq, n_cob);
   } else {
-    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
+    reg_dealloc<REG_AUX>();
+    if (warp == NUM_CONS / 32) {
+      // ================================================================ weight producer (1-D TMA bulk copies)
+      if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, W_STEP_BYTES, TPS, W_STAGE_BYTES, ntiles, n_tq, n_cob);
+    } else if (warp < (ST0 + NUM_STAGERS) / 32) {
+      stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
+    }
   }
 }
 
 // =============================================================================================
 // TIME-MAJOR variant for narrow layers (Cout <= 128; HiFi-GAN C = 64 / 32 stages, conv_post): the operand roles are
 // swapped --
-//     D[t (M = 64 frames per tile), co (N = NC / 2 per warpgroup)] = sum_tap sum_ci z[ci, t + tap*dil - pad] * W_tap[co, ci]
+//     D[t (M = 64 frames per warpgroup, 128 per tile), co (N = NC)] = sum_tap sum_ci z[ci, t + tap*dil - pad] * W_tap[co, ci]
 // The staged activation window is the A operand (same K-major 16-byte-row layout, a tap is still a descriptor shift), the
 // weights are the B operand with only NC = Cout rounded up to 32 (16 for Cout <= 16) rows: no tensor-pipe time and no weight
-// traffic is spent on absent output channels.  The two consumer warpgroups take one half of the channels each.  The
-// InstanceNorm partials of a channel are reduced over the warp's 16 frames with shuffles and over the four warps of a
-// warpgroup through shared memory (two passes: mean, then M2).  FAST recipe only.
+// traffic is spent on absent output channels.  The two consumer warpgroups take one half of the tile's frames each (warpgroup
+// 1's A descriptor starts 64 rows further into the staged window) and all NC channels; both read the whole weight stage.
+// The InstanceNorm partial of a channel over a warpgroup's 64 frames is reduced over the warp's 16 frames with shuffles and
+// over the four warps through shared memory (two passes: mean, then M2).  FAST recipe only.
 __host__ __device__ __forceinline__ int tmajor_nc(int Cout) { return Cout <= 16 ? 16 : ((Cout + 31) & ~31); }
 
 constexpr int T_WSTAGE = 16384;                           // bytes per weight stage: 16 taps (NC = 16) .. 2 taps (NC = 128)
 static_assert(T_WSTAGE <= W_STAGE_BYTES, "time-major stages live in the SM_W ring");
 
-template <int NH>   // channels per warpgroup = NC / 2
-__device__ __forceinline__ void tct_mma(float (&d)[NH / 2], float (&e)[NH / 2], uint64_t a0, uint64_t b0, uint64_t a1, uint64_t b1,
+template <int NC>   // output channels (weight rows) = wgmma N
+__device__ __forceinline__ void tct_mma(float (&d)[NC / 2], float (&e)[NC / 2], uint64_t a0, uint64_t b0, uint64_t a1, uint64_t b1,
                                         uint32_t acc) {
-  if constexpr (NH == 8) { wgmma_f16_n8(d, a0, b0, acc); wgmma_e4m3_n8(e, a1, b1, acc); }
-  else if constexpr (NH == 16) { wgmma_f16_n16(d, a0, b0, acc); wgmma_e4m3_n16(e, a1, b1, acc); }
-  else if constexpr (NH == 32) { wgmma_f16_n32(d, a0, b0, acc); wgmma_e4m3_n32(e, a1, b1, acc); }
-  else if constexpr (NH == 48) { wgmma_f16_n48(d, a0, b0, acc); wgmma_e4m3_n48(e, a1, b1, acc); }
-  else { wgmma_f16_n64(d, a0, b0, acc); wgmma_e4m3_n64(e, a1, b1, acc); }
+  if constexpr (NC == 16) { wgmma_f16_n16(d, a0, b0, acc); wgmma_e4m3_n16(e, a1, b1, acc); }
+  else if constexpr (NC == 32) { wgmma_f16_n32(d, a0, b0, acc); wgmma_e4m3_n32(e, a1, b1, acc); }
+  else if constexpr (NC == 64) { wgmma_f16_n64(d, a0, b0, acc); wgmma_e4m3_n64(e, a1, b1, acc); }
+  else if constexpr (NC == 96) { wgmma_f16_n96(d, a0, b0, acc); wgmma_e4m3_n96(e, a1, b1, acc); }
+  else { static_assert(NC == 128, "time-major N"); wgmma_f16_n128(d, a0, b0, acc); wgmma_e4m3_n128(e, a1, b1, acc); }
 }
 
-template <int NH>
+template <int NH>   // NC / 2
 __global__ void __launch_bounds__(THREADS, 1)
 conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int ncb, const int RW, const int ntiles, const int n_tq) {
   constexpr int MODE = MODE_FAST;
   constexpr int NC = 2 * NH;
-  constexpr int NJ = NH / 8;
+  constexpr int NJ = NC / 8;
+  static_assert(NC <= TCT_NC_MAX, "statistics scratch");
   const int RWP = RW + 2;
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = warp_uniform(tid), lane = tid & 31;
@@ -615,29 +684,30 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
   const int tps = T_WSTAGE / wstep;               // taps per weight stage: 1 (NC = 128, 96) .. 8 (NC = 16)
 
   if (warp < NUM_CONS / 32) {
+    reg_alloc<REG_CONS>();
     const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
     const bool leader = (tid & 127) == 0;
     const uint32_t lbo_x = (uint32_t)RWP * 16, lbo_w = (uint32_t)NC * 16;
     const uint32_t dil16 = (uint32_t)a.dil * 16u;
-    float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * 64;   // [4 warps][64 channels]
+    float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * TCT_NC_MAX;   // [4 warps][TCT_NC_MAX channels]
     int ws = 0, wph = 0, as = 0, aph = 0;
     Pending pend{-1, -1};
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int tq = tile % n_tq, b = tile / n_tq;
-      float d[NH / 2], e[NH / 2];   // fp16 main products / e4m3 correction products (e4m3 wgmma accumulates at reduced precision)
+      float d[NC / 2], e[NC / 2];   // fp16 main products / e4m3 correction products (e4m3 wgmma accumulates at reduced precision)
 #pragma unroll
-      for (int i = 0; i < NH / 2; ++i) { d[i] = 0.f; e[i] = 0.f; }
+      for (int i = 0; i < NC / 2; ++i) { d[i] = 0.f; e[i] = 0.f; }
       uint32_t acc = 0;
       for (int cb = 0; cb < ncb; ++cb) {
         mbar_wait(BAR(B_AFULL + as), aph);
-        uint32_t x_addr = sbase + SM_ACT + as * ACT_BUF_BYTES;
+        uint32_t x_addr = sbase + SM_ACT + as * ACT_BUF_BYTES + wg * TP * 16;   // warpgroup wg: frames TP wg .. of the tile
         for (int tap0 = 0; tap0 < K; tap0 += tps) {
           mbar_wait(BAR(B_WFULL + ws), wph);
           wg_fence();
           const int nt = min(tps, K - tap0);
-          uint32_t w_addr = sbase + SM_W + ws * T_WSTAGE + wg * NH * 16;
+          uint32_t w_addr = sbase + SM_W + ws * T_WSTAGE;
           for (int t = 0; t < nt; ++t) {
-            tct_mma<NH>(d, e, make_desc(x_addr, lbo_x, 128), make_desc(w_addr, lbo_w, 128), make_desc(x_addr + ACT_PLANE_BYTES, lbo_x, 128),
+            tct_mma<NC>(d, e, make_desc(x_addr, lbo_x, 128), make_desc(w_addr, lbo_w, 128), make_desc(x_addr + ACT_PLANE_BYTES, lbo_x, 128),
                         make_desc(w_addr + 2 * NC * 16, lbo_w, 128), acc);
             acc = 1;
             w_addr += wstep;
@@ -656,43 +726,63 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
       wg_fence_regs(d);
       wg_fence_regs(e);
 #pragma unroll
-      for (int i = 0; i < NH / 2; ++i) d[i] += e[i];
+      for (int i = 0; i < NC / 2; ++i) d[i] += e[i];
       release(bar0, pend, leader);
       pend.ws = -1;
 
-      // ---- epilogue: row = frame, column = output channel
-      const int t0 = tq * TN;
-      const int ncols = min(TN, a.Lq - t0);
+      // ---- epilogue: row = frame, column = output channel.  The warpgroup's 64 frames are one statistics partial; the
+      // second warpgroup of a tail tile can lie entirely beyond Lq (ncols <= 0): it then writes nothing.
+      const int t0 = tq * TN + wg * TP;
+      const int ncols = min(TP, a.Lq - t0);
       float* yb = a.y + (long long)b * a.y_bstride;
       const float* rbase = a.res ? a.res + (long long)b * a.res_bstride : nullptr;
       float s[NJ * 2], n[NJ * 2];
+      constexpr int G = NJ > 12 ? 1 : 2;   // channel groups of 8 per batch of loads; more spill at NC = 128 (192 registers)
 #pragma unroll
-      for (int j = 0; j < NJ; ++j) {
+      for (int j0 = 0; j0 < NJ; j0 += G) {
+        float bias[2 * G], res_v[4 * G], y_old[4 * G];   // operands of the group's elements first, then the stores (epi_load)
 #pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int co = wg * NH + 8 * j + 2 * t4 + c;
-          const bool cok = co < a.Cout;
-          const float bias = (a.bias && cok) ? a.bias[co] : 0.f;
-          float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-          const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
-          float ss = 0.f, nn = 0.f;
+        for (int jj = 0; jj < G; ++jj)
 #pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int fr = w * 16 + g + 8 * i;
-            const int r = 4 * j + 2 * i + c;
-            float val = 0.f;
-            if (cok && fr < ncols) {
-              val = epi_value(a, d[r] * D_UNSCALE, bias, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset);
-              ss += val;
-              nn += 1.f;
+          for (int c = 0; c < 2; ++c) {
+            const int co = 8 * (j0 + jj) + 2 * t4 + c;
+            const bool cok = co < a.Cout;
+            bias[2 * jj + c] = (a.bias && cok) ? a.bias[co] : 0.f;
+            const float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+            const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int fr = w * 16 + g + 8 * i;
+              epi_load(a, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset, cok && fr < ncols, res_v[4 * jj + 2 * i + c], y_old[4 * jj + 2 * i + c]);
             }
-            d[r] = val;
           }
-          s[2 * j + c] = ss;
-          n[2 * j + c] = nn;
+#pragma unroll
+        for (int jj = 0; jj < G; ++jj) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int j = j0 + jj, co = 8 * j + 2 * t4 + c;
+            const bool cok = co < a.Cout;
+            float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+            float ss = 0.f, nn = 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int fr = w * 16 + g + 8 * i;
+              const int r = 4 * j + 2 * i + c;
+              float val = 0.f;
+              if (cok && fr < ncols) {
+                val = epi_combine(a, d[r] * D_UNSCALE, bias[2 * jj + c], res_v[4 * jj + 2 * i + c], y_old[4 * jj + 2 * i + c]);
+                yp[(t0 + fr) * a.y_tstride + a.y_toffset] = val;
+                ss += val;
+                nn += 1.f;
+              }
+              d[r] = val;
+            }
+            s[2 * j + c] = ss;
+            n[2 * j + c] = nn;
+          }
         }
       }
-      if (a.stats) {
+      if (a.stats && ncols > 0) {
         const uint32_t bar_id = 3 + wg;
         // pass 1: sums over the 16 frames of the warp (lanes with equal t4), then over the warpgroup's four warps
 #pragma unroll
@@ -708,7 +798,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
 #pragma unroll
-            for (int c = 0; c < 2; ++c) red[w * 64 + 8 * j + 2 * t4 + c] = s[2 * j + c];
+            for (int c = 0; c < 2; ++c) red[w * TCT_NC_MAX + 8 * j + 2 * t4 + c] = s[2 * j + c];
         }
         asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
         float mean[2 * NJ], cnt[2 * NJ];
@@ -717,8 +807,8 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
 #pragma unroll
           for (int c = 0; c < 2; ++c) {
             const int ch = 8 * j + 2 * t4 + c;
-            const float tot = red[ch] + red[64 + ch] + red[128 + ch] + red[192 + ch];
-            // count of the tile = valid frames (the same for every existing channel)
+            const float tot = red[ch] + red[TCT_NC_MAX + ch] + red[2 * TCT_NC_MAX + ch] + red[3 * TCT_NC_MAX + ch];
+            // count of the partial = valid frames (the same for every existing channel)
             cnt[2 * j + c] = (float)max(0, ncols);
             mean[2 * j + c] = ncols > 0 ? tot / (float)ncols : 0.f;
           }
@@ -744,30 +834,34 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
 #pragma unroll
-            for (int c = 0; c < 2; ++c) red[w * 64 + 8 * j + 2 * t4 + c] = q[2 * j + c];
+            for (int c = 0; c < 2; ++c) red[w * TCT_NC_MAX + 8 * j + 2 * t4 + c] = q[2 * j + c];
         }
         asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");
         if (w == 0 && g == 0) {
+          const int part = tq * (TN / TP) + wg;
 #pragma unroll
           for (int j = 0; j < NJ; ++j)
 #pragma unroll
             for (int c = 0; c < 2; ++c) {
-              const int ch = 8 * j + 2 * t4 + c, co = wg * NH + ch;
+              const int co = 8 * j + 2 * t4 + c;
               if (co < a.Cout) {
-                float* gp = a.stats + (((long long)b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + tq) * 3;
+                float* gp = a.stats + (((long long)b * a.Cout + co) * a.stats_nparts + a.stats_part_offset + part) * 3;
                 gp[0] = cnt[2 * j + c];
                 gp[1] = mean[2 * j + c];
-                gp[2] = red[ch] + red[64 + ch] + red[128 + ch] + red[192 + ch];
+                gp[2] = red[co] + red[TCT_NC_MAX + co] + red[2 * TCT_NC_MAX + co] + red[3 * TCT_NC_MAX + co];
               }
             }
         }
       }
     }
-  } else if (warp == NUM_CONS / 32) {
-    // ================================================================ weight producer (1-D TMA bulk copies)
-    if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, wstep, tps, T_WSTAGE, ntiles, n_tq, 1);
   } else {
-    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, 1, tid, warp, lane);
+    reg_dealloc<REG_AUX>();
+    if (warp == NUM_CONS / 32) {
+      // ================================================================ weight producer (1-D TMA bulk copies)
+      if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, wstep, tps, T_WSTAGE, ntiles, n_tq, 1);
+    } else if (warp < (ST0 + NUM_STAGERS) / 32) {
+      stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, 1, tid, warp, lane);
+    }
   }
 }
 
@@ -1029,8 +1123,8 @@ int st2_conv1d_tc(const st2_conv_args* a, const void* wtc, int mode, int max_cta
   ST2_REQUIRE(st2_conv_tc_supported(a->Cin, a->Cout, a->K, a->stride, a->dil), "st2_conv1d_tc", "unsupported shape");
   ST2_REQUIRE(a->pre_act != ST2_ACT_SNAKE || a->pre_alpha, "st2_conv1d_tc", "snake prologue needs alpha");
   ST2_REQUIRE(!(mode & tc::TMAJOR) || a->dup_q0_to < 0, "st2_conv1d_tc", "time-major kernel: no reflection duplicate");
-  const int n_tq = cdiv(a->Lq, tc::TN);
-  ST2_REQUIRE(!a->stats || a->stats_nparts >= a->stats_part_offset + n_tq, "st2_conv1d_tc", "stats buffer too small (one partial per 64-column tile)");
+  const int nparts = cdiv(a->Lq, tc::TP);
+  ST2_REQUIRE(!a->stats || a->stats_nparts >= a->stats_part_offset + nparts, "st2_conv1d_tc", "stats buffer too small (one partial per 64 columns)");
   tc::launch_tc(*a, wtc, mode, max_ctas, (cudaStream_t)stream);
   ST2_CHECK_LAUNCH("st2_conv1d_tc");
   return 0;
@@ -1071,7 +1165,7 @@ int st2_conv_transpose1d_tc(const st2_conv_args* a0, const void* wtc, int mode, 
   ST2_REQUIRE(K > 0 && S > 0 && P >= 0, "st2_conv_transpose1d_tc", "bad shape");
   const int J = (K + S - 1) / S;
   ST2_REQUIRE(st2_conv_tc_supported(a0->Cin, a0->Cout, J, 1, 1), "st2_conv_transpose1d_tc", "unsupported shape");
-  const int parts = cdiv(a0->Lin, tc::TN);
+  const int parts = cdiv(a0->Lin, tc::TP);
   ST2_REQUIRE(!a0->stats || a0->stats_nparts >= S * parts, "st2_conv_transpose1d_tc", "stats buffer too small");
   const long long phase_bytes = st2_conv_tc_weight_bytes(a0->Cout, a0->Cin, J);
   for (int r = 0; r < S; ++r) {
