@@ -113,7 +113,13 @@ constexpr int SM_RAW = SM_ACT + 2 * ACT_BUF_BYTES;
 constexpr int SM_COEF = SM_RAW + RAW_STAGES * RAW_BYTES;
 constexpr int SM_EPI = SM_COEF + 4 * CIN_PAD_MAX * 4;   // per-channel prologue coefficients of the current utterance (4 x 1120 floats)
 constexpr int TCT_NC_MAX = 128;                   // output channels of the time-major kernel, max
-constexpr int SM_BAR = SM_EPI + 2 * 4 * TCT_NC_MAX * 4;   // time-major statistics scratch [2 warpgroups][4 warps][128 channels]
+constexpr int SM_SLOT = SM_EPI + 2 * 4 * TCT_NC_MAX * 4;   // time-major statistics scratch [2 warpgroups][4 warps][128 channels]
+// time-major epilogue slot: SLOT_Q float4 of folded accumulators per consumer thread; float4 q of consumer thread i lives at
+// (q * NUM_CONS + i) * 16 bytes (conflict-free), and a thread only ever reads back what it wrote itself.  The output
+// values are computed from here by a rolled loop: unrolled over the register fragments, they were ~4300 straight-line
+// instructions at NC = 128 (69 KB of code, run once per tile and so mostly from a cold instruction cache).
+constexpr int SLOT_Q = 8;
+constexpr int SM_BAR = SM_SLOT + SLOT_Q * NUM_CONS * 16;
 constexpr int SM_TOTAL = SM_BAR + 512;
 static_assert(RAW_CHUNKS % ST_PER_CH == 0 && NUM_STAGERS % 64 == 0 && NUM_STAGERS % CB == 0, "stager mappings");
 static_assert(RAW_CHUNKS * 4 >= RW_MAX + 3 && RAW_PITCH >= RAW_CHUNKS * 4 && (RAW_PITCH * 4) % 128 == 64, "raw window rows");
@@ -690,6 +696,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
     const uint32_t lbo_x = (uint32_t)RWP * 16, lbo_w = (uint32_t)NC * 16;
     const uint32_t dil16 = (uint32_t)a.dil * 16u;
     float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * TCT_NC_MAX;   // [4 warps][TCT_NC_MAX channels]
+    float4* slot = reinterpret_cast<float4*>(smem + SM_SLOT) + tid;              // this thread's float4 q at slot[q * NUM_CONS]
     int ws = 0, wph = 0, as = 0, aph = 0;
     Pending pend{-1, -1};
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -736,62 +743,94 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
       const int ncols = min(TP, a.Lq - t0);
       float* yb = a.y + (long long)b * a.y_bstride;
       const float* rbase = a.res ? a.res + (long long)b * a.res_bstride : nullptr;
-      float s[NJ * 2], n[NJ * 2];
-      constexpr int G = NJ > 12 ? 1 : 2;   // channel groups of 8 per batch of loads; more spill at NC = 128 (192 registers)
+      // residual / MRF operands of channel group j, loaded one group ahead of its stores (epi_load)
+      float res_n[4], old_n[4];
+      auto load_group = [&](int j) {
 #pragma unroll
-      for (int j0 = 0; j0 < NJ; j0 += G) {
-        float bias[2 * G], res_v[4 * G], y_old[4 * G];   // operands of the group's elements first, then the stores (epi_load)
+        for (int c = 0; c < 2; ++c) {
+          const int co = 8 * j + 2 * t4 + c;
+          const bool cok = co < a.Cout;
+          const float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+          const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
 #pragma unroll
-        for (int jj = 0; jj < G; ++jj)
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int co = 8 * (j0 + jj) + 2 * t4 + c;
-            const bool cok = co < a.Cout;
-            bias[2 * jj + c] = (a.bias && cok) ? a.bias[co] : 0.f;
-            const float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-            const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int fr = w * 16 + g + 8 * i;
-              epi_load(a, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset, cok && fr < ncols, res_v[4 * jj + 2 * i + c], y_old[4 * jj + 2 * i + c]);
-            }
-          }
-#pragma unroll
-        for (int jj = 0; jj < G; ++jj) {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int j = j0 + jj, co = 8 * j + 2 * t4 + c;
-            const bool cok = co < a.Cout;
-            float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-            float ss = 0.f, nn = 0.f;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int fr = w * 16 + g + 8 * i;
-              const int r = 4 * j + 2 * i + c;
-              float val = 0.f;
-              if (cok && fr < ncols) {
-                val = epi_combine(a, d[r] * D_UNSCALE, bias[2 * jj + c], res_v[4 * jj + 2 * i + c], y_old[4 * jj + 2 * i + c]);
-                yp[(t0 + fr) * a.y_tstride + a.y_toffset] = val;
-                ss += val;
-                nn += 1.f;
-              }
-              d[r] = val;
-            }
-            s[2 * j + c] = ss;
-            n[2 * j + c] = nn;
+          for (int i = 0; i < 2; ++i) {
+            const int fr = w * 16 + g + 8 * i;
+            epi_load(a, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset, cok && fr < ncols, res_n[2 * i + c], old_n[2 * i + c]);
           }
         }
+      };
+      // Output values, SLOT_Q channel groups at a time through the slot: float4 j - j0 holds frames w * 16 + g + {0, 8} (i)
+      // of channels 8 j + 2 t4 + {0, 1} (c) as components 2 i + c.  The loop over the groups stays rolled (compact code,
+      // see SM_SLOT); the values come back into the fragments for the statistics.
+#pragma unroll
+      for (int j0 = 0; j0 < NJ; j0 += SLOT_Q) {
+        constexpr int NQ = NJ < SLOT_Q ? NJ : SLOT_Q;   // NJ is 2, 4, 8, 12 or 16
+        const int nq = min(NQ, NJ - j0);
+#pragma unroll
+        for (int q = 0; q < NQ; ++q)
+          if (q < nq) slot[q * NUM_CONS] = make_float4(d[4 * (j0 + q)], d[4 * (j0 + q) + 1], d[4 * (j0 + q) + 2], d[4 * (j0 + q) + 3]);
+        load_group(j0);
+        auto value_group = [&](int j) {
+          float res_v[4], y_old[4];
+#pragma unroll
+          for (int k = 0; k < 4; ++k) { res_v[k] = res_n[k]; y_old[k] = old_n[k]; }
+          if (j + 1 < j0 + nq) load_group(j + 1);
+          const float4 qv = slot[(j - j0) * NUM_CONS];
+          const float v[4] = {qv.x, qv.y, qv.z, qv.w};
+          float o[4];
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int co = 8 * j + 2 * t4 + c;
+            const bool cok = co < a.Cout;
+            float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
+            const float bias = (a.bias && cok) ? __ldg(a.bias + co) : 0.f;
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const int fr = w * 16 + g + 8 * i;
+              float val = 0.f;
+              if (cok && fr < ncols) {
+                val = epi_combine(a, v[2 * i + c] * D_UNSCALE, bias, res_v[2 * i + c], y_old[2 * i + c]);
+                yp[(t0 + fr) * a.y_tstride + a.y_toffset] = val;
+              }
+              o[2 * i + c] = val;
+            }
+          }
+          slot[(j - j0) * NUM_CONS] = make_float4(o[0], o[1], o[2], o[3]);
+        };
+        if constexpr (NJ > 4) {
+#pragma unroll 1
+          for (int j = j0; j < j0 + nq; ++j) value_group(j);
+        } else {   // NC <= 32: short enough unrolled (rolled, ptxas spills in the stager warps of NC = 32)
+#pragma unroll
+          for (int j = j0; j < j0 + nq; ++j) value_group(j);
+        }
+#pragma unroll
+        for (int q = 0; q < NQ; ++q)
+          if (q < nq) {
+            const float4 qv = slot[q * NUM_CONS];
+            d[4 * (j0 + q)] = qv.x; d[4 * (j0 + q) + 1] = qv.y; d[4 * (j0 + q) + 2] = qv.z; d[4 * (j0 + q) + 3] = qv.w;
+          }
       }
+      // per-thread sums of each channel over its two frames, in the order the values were produced
+      float s[NJ * 2];
+#pragma unroll
+      for (int j = 0; j < NJ; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const bool cok = 8 * j + 2 * t4 + c < a.Cout;
+          float ss = 0.f;
+#pragma unroll
+          for (int i = 0; i < 2; ++i)
+            if (cok && w * 16 + g + 8 * i < ncols) ss += d[4 * j + 2 * i + c];
+          s[2 * j + c] = ss;
+        }
       if (a.stats && ncols > 0) {
         const uint32_t bar_id = 3 + wg;
         // pass 1: sums over the 16 frames of the warp (lanes with equal t4), then over the warpgroup's four warps
 #pragma unroll
         for (int k = 0; k < 2 * NJ; ++k) {
 #pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
-            n[k] += __shfl_xor_sync(0xffffffffu, n[k], o);
-          }
+          for (int o = 4; o < 32; o <<= 1) s[k] += __shfl_xor_sync(0xffffffffu, s[k], o);
         }
         asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory");   // the previous tile's readers are done
         if (g == 0) {
