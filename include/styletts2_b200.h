@@ -185,10 +185,16 @@ typedef struct st2_rows_args {
   const int* lengths;     /* rows n >= lengths[b] are written as zeros (masked_fill), may be NULL */
 } st2_rows_args;
 int st2_rows_ln(const st2_rows_args* a, void* stream);
+/* The same per-row work over M packed token rows (only the valid rows of every utterance, concatenated): the utterance of
+ * row r is row_utt[r] (int32 [M]), which selects x, add and the per-utterance g/b rows; a->N and a->lengths are unused. */
+int st2_rows_ln_packed(const st2_rows_args* a, const int* row_utt, int M, void* stream);
 /* dst[(b,n), col0 + j] = (n < lengths[b]) ? src[b, j] : 0   (style concat, models.py:539-541,551-552) */
 int st2_bcast_cols(float* dst, long long ld, int col0, const float* src, int B, int N, int W, const int* lengths, void* stream);
 /* out[b,:] = mean_n h[(b,n),:]  (modules.py:399) */
 int st2_mean_rows(const float* h, long long ld, int B, int N, int C, float* out, void* stream);
+/* out[b,:] = mean of rows offsets[b] .. offsets[b+1]-1 of h (packed rows, offsets int32 [B+1], every segment non-empty);
+ * the summation order of st2_mean_rows, so equal segments give identical bits. */
+int st2_mean_segments(const float* h, long long ld, const int* offsets, int B, int C, float* out, void* stream);
 
 /* C[M,Nf] = act(A W^T + bias) + R.  A element (m,k): A + (m / a_L)*a_bs + (m % a_L)*a_ls + k*a_ks
  * (row layout: a_L=M, a_ls=K, a_ks=1; conv layout [B,K,L]: a_L=L, a_bs=K*L, a_ls=1, a_ks=L).
@@ -238,6 +244,12 @@ int st2_attention_ex(const float* q, long long q_ld, const float* k, const float
 int st2_attention_tc_supported(long long q_ld, long long kv_ld, long long out_ld, int D);
 int st2_attention_tc(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out, long long out_ld,
                      const int* lengths, int B, int N, int H, int D, float scale, void* stream);
+/* The same kernel on packed rows: utterance b owns rows offsets[b] .. offsets[b+1]-1 of q, k, v and out (offsets int32
+ * [B+1], every n_b = offsets[b+1] - offsets[b] >= 1, max_len >= every n_b).  Attention stays inside each utterance's rows;
+ * rows of other utterances are neither read as keys nor written.  Grid (ceil(max_len/64), H, B).  With offsets[b] = b*N it
+ * computes the bits of st2_attention_tc(lengths = NULL).  The range flag sees valid rows and keys only. */
+int st2_attention_tc_packed(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out,
+                            long long out_ld, const int* offsets, int B, int max_len, int H, int D, float scale, void* stream);
 /* ALBERT embeddings: out[(b,n), :] = word[tokens[b,n]] + pos[n] + type0   (E columns) */
 int st2_embedding_sum_rows(const long long* tokens, const float* word, const float* pos, const float* type0, int B, int N, int E,
                            float* out, void* stream);

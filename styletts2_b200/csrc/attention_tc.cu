@@ -21,6 +21,12 @@
 // range flag (as linear_tc.cu does), which st2_range_flag_fetch() reports and clears.  Masked keys and padded query rows
 // are staged as zeros and never raise it.  Every length must be >= 1: with no valid key the row sum is 0 and the output
 // non-finite (the SIMT kernel st2_attention_ex gives NaN there too).
+//
+// Packed rows (PACKED = true, st2_attention_tc_packed): utterance b owns rows offsets[b] .. offsets[b+1] - 1 of q / k / v /
+// out, concatenated without padding (varlen layout).  The kernel body is the same with N = n_b and the row base taken from
+// the offsets: rows and keys are clamped to the utterance's last row, keys >= n_b are masked, query rows >= n_b (the next
+// utterance's rows) are never stored, and a CTA whose query block starts at or beyond n_b exits.  With offsets[b] = b * N
+// it does the arithmetic of the padded kernel with lengths = NULL.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -55,9 +61,10 @@ struct Args {
   const float* q; long long q_ld;
   const float* k; const float* v; long long kv_ld;
   float* out; long long out_ld;
-  const int* lengths;
+  const int* lengths;      // key lengths [B] or NULL (padded layout)
   int N, H;
   float scale;
+  const int* offsets;      // row offsets [B + 1] (packed layout)
 };
 
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& p0, uint32_t& p1) {
@@ -86,15 +93,17 @@ __device__ __forceinline__ void load8(const float* p, float (&x)[8]) {
   x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
 }
 
+template <bool PACKED>
 __global__ void __launch_bounds__(THREADS, 1) attention_tc_kernel(const Args a) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, w = tid >> 5, lane = tid & 31, g = lane >> 2, t4 = lane & 3;
   const uint32_t sbase = smem_u32(smem);
   const int qb = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int N = a.N;
-  const int klen = a.lengths ? min(a.lengths[b], N) : N;
+  const int N = PACKED ? a.offsets[b + 1] - a.offsets[b] : a.N;     // rows of this utterance
+  if (PACKED && qb * QB >= N) return;
+  const int klen = PACKED ? N : (a.lengths ? min(a.lengths[b], N) : N);
   const int nkb = max(1, (klen + KB - 1) / KB);
-  const long long rowbase = (long long)b * N;
+  const long long rowbase = PACKED ? (long long)a.offsets[b] : (long long)b * N;
   bool in_range = true;
 
   // ---- stage Q (once): thread t -> query row t % 64, four 8-wide chunks of d
@@ -288,16 +297,41 @@ int st2_attention_tc(const float* q, long long q_ld, const float* k, const float
   cudaGetDevice(&dev);
   dev &= 63;
   if (!attr_done[dev]) {
-    cudaFuncSetAttribute(atc::attention_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, atc::SM_TOTAL);
+    cudaFuncSetAttribute(atc::attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc::SM_TOTAL);
     attr_done[dev] = true;
   }
   atc::Args a;
-  a.q = q; a.q_ld = q_ld; a.k = k; a.v = v; a.kv_ld = kv_ld; a.out = out; a.out_ld = out_ld; a.lengths = lengths;
+  a.q = q; a.q_ld = q_ld; a.k = k; a.v = v; a.kv_ld = kv_ld; a.out = out; a.out_ld = out_ld; a.lengths = lengths; a.offsets = nullptr;
   a.N = N; a.H = H; a.scale = scale;
   dim3 grid(cdiv(N, atc::QB), H, B);
-  atc::attention_tc_kernel<<<grid, atc::THREADS, atc::SM_TOTAL, (cudaStream_t)stream>>>(a);
+  atc::attention_tc_kernel<false><<<grid, atc::THREADS, atc::SM_TOTAL, (cudaStream_t)stream>>>(a);
   ++g_launches;
   ST2_CHECK_LAUNCH("st2_attention_tc");
+  return 0;
+}
+
+int st2_attention_tc_packed(const float* q, long long q_ld, const float* k, const float* v, long long kv_ld, float* out,
+                            long long out_ld, const int* offsets, int B, int max_len, int H, int D, float scale, void* stream) {
+  ST2_REQUIRE(q && k && v && out && offsets && B > 0 && max_len > 0 && H > 0, "st2_attention_tc_packed", "bad args");
+  ST2_REQUIRE(st2_attention_tc_supported(q_ld, kv_ld, out_ld, D), "st2_attention_tc_packed",
+              "head_features must be 64, row strides multiples of 4");
+  ST2_REQUIRE(((reinterpret_cast<size_t>(q) | reinterpret_cast<size_t>(k) | reinterpret_cast<size_t>(v) | reinterpret_cast<size_t>(out)) & 15) == 0,
+              "st2_attention_tc_packed", "pointers must be 16-byte aligned");
+  static bool attr_done[64] = {false};
+  int dev = 0;
+  cudaGetDevice(&dev);
+  dev &= 63;
+  if (!attr_done[dev]) {
+    cudaFuncSetAttribute(atc::attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, atc::SM_TOTAL);
+    attr_done[dev] = true;
+  }
+  atc::Args a;
+  a.q = q; a.q_ld = q_ld; a.k = k; a.v = v; a.kv_ld = kv_ld; a.out = out; a.out_ld = out_ld; a.lengths = nullptr; a.offsets = offsets;
+  a.N = max_len; a.H = H; a.scale = scale;
+  dim3 grid(cdiv(max_len, atc::QB), H, B);
+  atc::attention_tc_kernel<true><<<grid, atc::THREADS, atc::SM_TOTAL, (cudaStream_t)stream>>>(a);
+  ++g_launches;
+  ST2_CHECK_LAUNCH("st2_attention_tc_packed");
   return 0;
 }
 

@@ -7,12 +7,14 @@ extern long long g_launches;
 
 // ------------------------------------------------------------------------------------------
 // rows_ln: one warp per row, row kept in registers (C <= 1024, C % 32 == 0).
-__global__ void __launch_bounds__(256) rows_ln_kernel(const st2_rows_args a) {
+// PACKED: M packed token rows, the utterance of row r is row_utt[r] (no padding rows, so nothing is masked).
+template <bool PACKED>
+__global__ void __launch_bounds__(256) rows_ln_kernel(const st2_rows_args a, const int* __restrict__ row_utt, int M) {
   const int lane = threadIdx.x & 31;
   const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= a.B * a.N) return;
-  const int b = row / a.N, n = row - b * a.N;
-  const bool masked = a.lengths && n >= a.lengths[b];
+  if (row >= (PACKED ? M : a.B * a.N)) return;
+  const int b = PACKED ? row_utt[row] : row / a.N;
+  const bool masked = !PACKED && a.lengths && row - b * a.N >= a.lengths[b];
   const int per = a.C >> 5;
   float v[32];
   float s = 0.f;
@@ -79,6 +81,19 @@ __global__ void mean_rows_kernel(const float* __restrict__ h, long long ld, int 
   float s = 0.f;
   for (int n = 0; n < N; ++n) s += p[(long long)n * ld];
   out[(long long)b * C + c] = s / (float)N;
+}
+
+// out[b,c] = mean of rows offsets[b] .. offsets[b+1]-1 of h; the summation order of mean_rows_kernel.
+__global__ void mean_segments_kernel(const float* __restrict__ h, long long ld, const int* __restrict__ offsets, int C,
+                                     float* __restrict__ out) {
+  const int b = blockIdx.y;
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const int r0 = offsets[b], n_b = offsets[b + 1] - r0;
+  const float* p = h + (long long)r0 * ld + c;
+  float s = 0.f;
+  for (int n = 0; n < n_b; ++n) s += p[(long long)n * ld];
+  out[(long long)b * C + c] = s / (float)n_b;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -435,9 +450,19 @@ int st2_rows_ln(const st2_rows_args* a, void* stream) {
   ST2_REQUIRE(a && (a->h_in || (a->x && a->emb)), "st2_rows_ln", "no input");
   ST2_REQUIRE(a->C % 32 == 0 && a->C <= 1024 && a->C > 0 && a->B > 0 && a->N > 0, "st2_rows_ln", "C must be a multiple of 32, <= 1024");
   const int rows = a->B * a->N;
-  rows_ln_kernel<<<cdiv(rows, 8), 256, 0, (cudaStream_t)stream>>>(*a);
+  rows_ln_kernel<false><<<cdiv(rows, 8), 256, 0, (cudaStream_t)stream>>>(*a, nullptr, 0);
   ++g_launches;
   ST2_CHECK_LAUNCH("st2_rows_ln");
+  return 0;
+}
+
+int st2_rows_ln_packed(const st2_rows_args* a, const int* row_utt, int M, void* stream) {
+  ST2_REQUIRE(a && (a->h_in || (a->x && a->emb)), "st2_rows_ln_packed", "no input");
+  ST2_REQUIRE(row_utt && M > 0 && a->B > 0, "st2_rows_ln_packed", "bad args");
+  ST2_REQUIRE(a->C % 32 == 0 && a->C <= 1024 && a->C > 0, "st2_rows_ln_packed", "C must be a multiple of 32, <= 1024");
+  rows_ln_kernel<true><<<cdiv(M, 8), 256, 0, (cudaStream_t)stream>>>(*a, row_utt, M);
+  ++g_launches;
+  ST2_CHECK_LAUNCH("st2_rows_ln_packed");
   return 0;
 }
 
@@ -456,6 +481,14 @@ int st2_mean_rows(const float* h, long long ld, int B, int N, int C, float* out,
   mean_rows_kernel<<<dim3(cdiv(C, 128), B), 128, 0, (cudaStream_t)stream>>>(h, ld, N, C, out);
   ++g_launches;
   ST2_CHECK_LAUNCH("st2_mean_rows");
+  return 0;
+}
+
+int st2_mean_segments(const float* h, long long ld, const int* offsets, int B, int C, float* out, void* stream) {
+  ST2_REQUIRE(h && offsets && out && B > 0 && C > 0, "st2_mean_segments", "bad args");
+  mean_segments_kernel<<<dim3(cdiv(C, 128), B), 128, 0, (cudaStream_t)stream>>>(h, ld, offsets, C, out);
+  ++g_launches;
+  ST2_CHECK_LAUNCH("st2_mean_segments");
   return 0;
 }
 

@@ -7,6 +7,14 @@
     STinference(text, ref_s, ref_text, alpha, beta, diffusion_steps, embedding_scale)  Demo/Inference_LibriTTS.ipynb#cell45
     compute_style(wave or path)                                                        Demo/Inference_LibriTTS.ipynb#cell5
 
+and one batched call with the `inference` signature over a list of texts (no notebook counterpart):
+
+    inference_batch(texts, noise [B,1,256], diffusion_steps=5, embedding_scale=1)                   single-speaker
+    inference_batch(texts, ref_s [B,256], alpha=0.3, beta=0.7, diffusion_steps=5, embedding_scale=1)  multispeaker
+
+which returns one waveform per text, each what `inference` gives for that text alone (the style sampler runs on packed
+token rows, Synthesizer.synthesize_texts).
+
 The notebooks define these as module-level functions over globals (`model`, `sampler`, `textclenaer`,
 `global_phonemizer`, `device`); `bind(...)` builds the same set of callables over a `build_model()` container of this
 package, so a notebook swaps its import and keeps its cells:
@@ -68,8 +76,8 @@ def bind(model: Munch, model_params, device="cuda", phonemizer=None, word_tokeni
         with torch.no_grad():
             return model.bert(tk, attention_mask=(~mask).int())
 
-    def _noise():
-        return torch.randn((1, 256)).unsqueeze(1).to(dev)          # the multispeaker cells draw it themselves
+    def _noise(B=1):
+        return torch.randn((B, 256)).unsqueeze(1).to(dev)          # the multispeaker cells draw it themselves
 
     if not multispeaker:
         def inference(text, noise, diffusion_steps=5, embedding_scale=1):
@@ -81,8 +89,17 @@ def bind(model: Munch, model_params, device="cuda", phonemizer=None, word_tokeni
             return syn.LFinference(tokens, _bert(tokens), s_prev, noise=noise, t=alpha, diffusion_steps=diffusion_steps,
                                    embedding_scale=embedding_scale)
 
+        def inference_batch(texts, noise, diffusion_steps=5, embedding_scale=1):
+            token_lists = [_tokens(t, strip_quotes=True) for t in texts]
+            return syn.synthesize_texts(token_lists, noise=noise, diffusion_steps=diffusion_steps, embedding_scale=embedding_scale)
+
         STinference = None
     else:
+        def inference_batch(texts, ref_s, alpha=0.3, beta=0.7, diffusion_steps=5, embedding_scale=1):
+            token_lists = [_tokens(t, strip_quotes=False) for t in texts]
+            return syn.synthesize_texts(token_lists, noise=_noise(len(texts)), ref_s=ref_s, alpha=alpha, beta=beta,
+                                        diffusion_steps=diffusion_steps, embedding_scale=embedding_scale)
+
         def inference(text, ref_s, alpha=0.3, beta=0.7, diffusion_steps=5, embedding_scale=1):
             tokens = _tokens(text, strip_quotes=False)
             return syn.inference(tokens, _bert(tokens), noise=_noise(), ref_s=ref_s, alpha=alpha, beta=beta,
@@ -112,6 +129,6 @@ def bind(model: Munch, model_params, device="cuda", phonemizer=None, word_tokeni
         wave = torch.as_tensor(np.asarray(wave_or_path), dtype=torch.float32)
         return _cs(model, wave.to(dev))
 
-    return Munch(inference=inference, LFinference=LFinference, STinference=STinference, compute_style=compute_style,
+    return Munch(inference=inference, inference_batch=inference_batch, LFinference=LFinference, STinference=STinference, compute_style=compute_style,
                  textclenaer=textclenaer, length_to_mask=length_to_mask, sampler=make_sampler(model), synthesizer=syn,
                  device=dev, global_phonemizer=global_phonemizer, word_tokenize=wt)

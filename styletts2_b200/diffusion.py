@@ -40,6 +40,36 @@ class FixedEmbedding(nn.Module):
         return self.embedding.weight[:N].unsqueeze(0).expand(B, -1, -1)
 
 
+class TokenPacking:
+    """Packed token rows of a batch: only the valid rows of every utterance, concatenated (varlen layout).  Utterance b
+    owns rows offsets[b] .. offsets[b+1]-1; row r belongs to utterance row_utt[r] at position pos[r].  The denoiser run on
+    this layout confines attention and the token mean to each utterance's own rows, so every utterance gets the style it
+    gets when it runs alone, whatever the other token counts of the batch."""
+
+    def __init__(self, lengths, device):
+        lengths = [int(n) for n in lengths]
+        assert lengths and min(lengths) >= 1, lengths
+        self.lengths = lengths
+        self.B, self.M, self.max_len = len(lengths), sum(lengths), max(lengths)
+        offs = [0]
+        for n in lengths:
+            offs.append(offs[-1] + n)
+        utt = torch.repeat_interleave(torch.arange(self.B), torch.tensor(lengths))
+        pos = torch.cat([torch.arange(n) for n in lengths])
+        self.offsets = torch.tensor(offs, dtype=torch.int32).to(device)
+        self.row_utt = utt.to(device=device, dtype=torch.int32)
+        self._utt, self._pos = utt.to(device), pos.to(device)
+
+    def pack(self, x):
+        """[B, N, ...] (N >= every length) -> [M, ...] contiguous: the valid rows, utterance after utterance"""
+        return x[self._utt, self._pos].contiguous()
+
+    def pack_positions(self, table):
+        """[L, ...] per-position table -> [M, ...]: row r takes table[r - offsets[b]] (the fixed embedding under guidance)"""
+        assert self.max_len <= table.shape[0], "Input sequence length must be <= max_length"
+        return table[self._pos].contiguous()
+
+
 class AttentionBase(nn.Module):
     def __init__(self, features, *, head_features, num_heads, out_features=None):
         super().__init__()
@@ -105,19 +135,33 @@ class Transformer1d(nn.Module):
         m = self.to_mapping[0](m, act=ACT_GELU)
         return self.to_mapping[2](m, act=ACT_GELU)
 
-    def run(self, x, time, embedding, features):
-        B, N, E = embedding.shape
+    def run(self, x, time, embedding, features, packed=None):
+        """embedding [B, N, E]; or, with packed = (offsets, row_utt, max_len), the packed token rows [M, E] of a
+        TokenPacking (see run_packed)"""
+        H, D = self.num_heads, self.head_features
+        if packed is None:
+            B, N, E = embedding.shape
+            M = B * N
+            emb = embedding if embedding.stride(-1) == 1 and embedding.stride(0) == N * embedding.stride(1) else embedding.contiguous()
+            rows_ln = lambda **kw: ops.rows_ln(B=B, N=N, **kw)                   # noqa: E731
+            attention = lambda q, kv: ops.attention(q, kv, B, N, H, D)           # noqa: E731
+            mean = lambda h: ops.mean_rows(h, B, N)                              # noqa: E731
+        else:
+            offsets, row_utt, max_len = packed
+            M, E = embedding.shape
+            B = offsets.shape[0] - 1
+            emb = embedding if embedding.stride(-1) == 1 else embedding.contiguous()
+            rows_ln = lambda **kw: ops.rows_ln_packed(row_utt=row_utt, M=M, B=B, **kw)             # noqa: E731
+            attention = lambda q, kv: ops.attention_packed(q, kv, offsets, B, max_len, H, D)     # noqa: E731
+            mean = lambda h: ops.mean_segments(h, offsets, B)                                    # noqa: E731
         dev = embedding.device
         Cw = self.features
-        M = B * N
         mapping = self.get_mapping(time, features)
-        emb = embedding if embedding.stride(-1) == 1 and embedding.stride(0) == N * embedding.stride(1) else embedding.contiguous()
         x2 = x.reshape(B, self.channels).contiguous()
         h = ops.empty(M, Cw, device=dev)
         a = ops.empty(M, Cw, device=dev)
         c = ops.empty(M, Cw, device=dev)
         feats = features.contiguous() if features is not None else None
-        H, D = self.num_heads, self.head_features
         for i, blk in enumerate(self.blocks):
             att = blk.attention
             if self.style:
@@ -126,19 +170,24 @@ class Transformer1d(nn.Module):
             else:
                 kw = dict(g1=att.norm.weight, b1=att.norm.bias, g2=att.norm_context.weight, b2=att.norm_context.bias)
             if i == 0:
-                ops.rows_ln(B=B, N=N, Cw=Cw, x=x2, xs=1.0, emb=emb, add=mapping, h_out=h, out1=a, out2=c, eps=1e-5, **kw)
+                rows_ln(Cw=Cw, x=x2, xs=1.0, emb=emb, add=mapping, h_out=h, out1=a, out2=c, eps=1e-5, **kw)
             else:
-                ops.rows_ln(B=B, N=N, Cw=Cw, h_in=h, add=mapping, h_out=h, out1=a, out2=c, eps=1e-5, **kw)
+                rows_ln(Cw=Cw, h_in=h, add=mapping, h_out=h, out1=a, out2=c, eps=1e-5, **kw)
             q = att.to_q(a)
             kv = att.to_kv(c)
-            o = ops.attention(q, kv, B, N, H, D)
+            o = attention(q, kv)
             att.attention.to_out(o, R=h, out=h)
             f = blk.feed_forward[0](h, act=ACT_GELU)
             blk.feed_forward[2](f, R=h, out=h)
-        hm = ops.mean_rows(h, B, N)
+        hm = mean(h)
         conv = self.to_out[1]
         out = ops.linear(hm, conv.weight.view(conv.cout, conv.cin), conv.bias)
         return out.view(B, 1, self.channels)
+
+    def run_packed(self, x, time, embedding, features, offsets, row_utt, max_len):
+        """x [B,1,C], embedding [M,E] packed token rows (TokenPacking.pack), offsets int32 [B+1], row_utt int32 [M] ->
+        [B,1,C]: each utterance attends over and averages its own rows only (the single-utterance result)"""
+        return self.run(x, time, embedding, features, packed=(offsets, row_utt, max_len))
 
     def forward(self, x, time, embedding_mask_proba: float = 0.0, embedding=None, features=None, embedding_scale: float = 1.0):
         assert embedding_mask_proba == 0.0, "inference path only (no conditional dropout)"
@@ -264,6 +313,10 @@ class _DenoiseEval:
 
     def __init__(self, diffusion: KDiffusion, kwargs):
         self.kd, self.kw = diffusion, kwargs
+        self.packing = kwargs.get("packing")        # TokenPacking: `embedding` holds its packed rows [M, 768]
+        self.fixed_packed = None
+        if self.packing is not None and kwargs.get("embedding_scale", 1.0) != 1.0:
+            self.fixed_packed = self.packing.pack_positions(diffusion.net.fixed_embedding.embedding.weight)
 
     def step(self, x_eval, sigma_eval, x_base, dt, eps=None, sigma_up=0.0):
         kd = self.kd
@@ -274,10 +327,18 @@ class _DenoiseEval:
         net = kd.net
         emb, feats = self.kw.get("embedding"), self.kw.get("features")
         scale = self.kw.get("embedding_scale", 1.0)
-        pred = net.run(xin, t, emb, feats)
-        masked = None
-        if scale != 1.0:
-            masked = net.run(xin, t, net.fixed_embedding(emb).contiguous(), feats)
+        pk = self.packing
+        if pk is not None:
+            packed = (pk.offsets, pk.row_utt, pk.max_len)
+            pred = net.run_packed(xin, t, emb, feats, *packed)
+            masked = None
+            if scale != 1.0:
+                masked = net.run_packed(xin, t, self.fixed_packed, feats, *packed)
+        else:
+            pred = net.run(xin, t, emb, feats)
+            masked = None
+            if scale != 1.0:
+                masked = net.run(xin, t, net.fixed_embedding(emb).contiguous(), feats)
         return ops.kdiff_step(x_eval, pred.reshape(x_eval.shape), c_skip, c_out, float(torch.tensor(sigma_eval, dtype=torch.float32)),
                               x_base, dt, eps=eps, sigma_up=sigma_up,
                               x_pred_masked=None if masked is None else masked.reshape(x_eval.shape), cfg_scale=scale)

@@ -14,7 +14,7 @@ from typing import Dict, List, Optional
 import torch
 
 from . import ops
-from .diffusion import ADPM2Sampler, DiffusionSampler, KarrasSchedule
+from .diffusion import ADPM2Sampler, DiffusionSampler, KarrasSchedule, TokenPacking
 from .models import Munch
 
 
@@ -86,7 +86,8 @@ class Synthesizer:
     @torch.no_grad()
     def synthesize(self, tokens, input_lengths, bert_dur, noise, *, diffusion_steps=5, embedding_scale=1.0, ref_s=None,
                    alpha=0.3, beta=0.7, rng: Optional[Dict] = None, forced_durations=None, pin_frames_per_token=None,
-                   return_all=False, decoder_events=None, stage_marks=None, s_prev=None, t=0.7, last_plus=None):
+                   return_all=False, decoder_events=None, stage_marks=None, s_prev=None, t=0.7, last_plus=None,
+                   token_packing=False):
         """tokens [B,N] i64, input_lengths [B], bert_dur [B,N,768] (or None: model.bert runs), noise [B,1,256] (device tensors).
         rng (parity mode): 'step_noises' list of [B,1,256], 'sine_noise' [B,L,9], 'har' [B,22,F],
         'F0' / 'N' [B,2T] (teacher-forced prosody curves: the harmonic source integrates F0 into a phase
@@ -96,6 +97,11 @@ class Synthesizer:
         pin_frames_per_token: throughput mode of SURVEY section 8d (durations pinned so that T = N*k).
         last_plus: frames added to the last real token (None: 5 single-speaker / 0 multispeaker as the notebooks'
         `inference`; LFinference of the LJSpeech notebook passes 0).
+        token_packing: run the style sampler on packed token rows (diffusion.TokenPacking): each utterance's denoiser
+        attends over and averages its own tokens only, so its s_pred is the one it gets alone, whatever the token counts
+        of the rest of the batch.  Off (the default), the sampler sees the padded batch as the reference's batched
+        sampler does: padding an utterance changes its style.  The packed path reads input_lengths on the host (one sync)
+        and cannot be captured into a CUDA graph.
         s_prev [B,256], t: long-form style carry-over of the notebooks' LFinference (LJSpeech cell 29, LibriTTS cell 42):
         s_pred = t*s_prev + (1-t)*s_pred before it is split; out['s_carry'] is the value to pass as the next s_prev."""
         m = self.model
@@ -119,6 +125,10 @@ class Synthesizer:
         with _stage("sampler", marks):
             kw = dict(embedding=bert_dur, num_steps=diffusion_steps, embedding_scale=embedding_scale,
                       step_noises=rng.get("step_noises"))
+            if token_packing:
+                packing = TokenPacking(input_lengths.tolist(), dev)     # host lengths size the packed buffers
+                assert packing.B == B and packing.max_len <= N, (input_lengths, N)
+                kw.update(embedding=packing.pack(bert_dur), packing=packing)
             if self.multispeaker:
                 kw["features"] = ref_s
             s_pred = self.sampler(noise, **kw).reshape(B, 256)
@@ -244,6 +254,33 @@ class Synthesizer:
             st["ref_s"].copy_(ref_s, non_blocking=True)
         ent["graph"].replay()
         return ent["wav"], ent["launches"]
+
+    @torch.no_grad()
+    def synthesize_texts(self, token_lists: List[List[int]], noise=None, ref_s=None, bert_dur=None, **kw):
+        """A batch of utterances with any token counts in one call, each with the notebooks' single-utterance `inference`
+        result: the token lists (already cleaned, with the leading 0) are padded, the text side runs batched with the style
+        sampler on packed token rows (token_packing=True), and one numpy waveform per utterance comes back (LJSpeech: last
+        token +5 frames; LibriTTS: the last 50 samples cut).  After the durations the batch is grouped by total frame count
+        and each group runs its own prosody / decoder launch chain.
+        noise [B,1,256] (None: drawn on the device), ref_s [B,256] or [1,256] (multispeaker), bert_dur [B,N,768] padded PL-BERT output
+        (None: model.bert runs on the padded batch with its attention mask); kw go to synthesize."""
+        dev = self.device
+        B = len(token_lists)
+        lens = [len(t) for t in token_lists]
+        N = max(lens)
+        tk = torch.zeros(B, N, dtype=torch.long)
+        for b, t in enumerate(token_lists):
+            tk[b, :lens[b]] = torch.as_tensor(list(t), dtype=torch.long)
+        if noise is None:
+            noise = ops.randn_like(torch.empty(B, 1, 256, device=dev))
+        if ref_s is not None:
+            ref_s = ref_s.to(dev).reshape(-1, 256).expand(B, 256).contiguous()     # one row: the same voice for all
+        out = self.synthesize(tk.to(dev), torch.tensor(lens, device=dev), None if bert_dur is None else bert_dur.to(dev),
+                              noise.to(dev).reshape(B, 1, 256), ref_s=ref_s, token_packing=True, **kw)
+        wav = out["wav"].reshape(B, -1).cpu().numpy()
+        wl = out["wav_lengths"].tolist()
+        wavs = [wav[b, :wl[b]] for b in range(B)]
+        return [w[..., :-50] for w in wavs] if self.multispeaker else wavs
 
     # ------------------------------------------------------------------ single-utterance conveniences (token ids in)
     def _one(self, tokens: List[int], bert_dur, noise, **kw):

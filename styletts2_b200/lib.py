@@ -85,6 +85,8 @@ SIGNATURES = {
     "st2_rows_ln": [C.POINTER(RowsArgs), _vp],
     "st2_bcast_cols": [_vp, _ll, _i, _vp, _i, _i, _i, _vp, _vp],
     "st2_mean_rows": [_vp, _ll, _i, _i, _i, _vp, _vp],
+    "st2_rows_ln_packed": [C.POINTER(RowsArgs), _vp, _i, _vp],
+    "st2_mean_segments": [_vp, _ll, _vp, _i, _i, _vp, _vp],
     "st2_linear": [_vp, _ll, _ll, _ll, _i, _vp, _vp, _vp, _ll, _vp, _ll, _i, _i, _i, _i, _vp],
     "st2_linear_tc_weight_bytes": [_i, _i],
     "st2_linear_tc_weight_layout": [_vp, _vp, _i, _i, _vp],
@@ -97,6 +99,7 @@ SIGNATURES = {
     "st2_attention_ex": [_vp, _ll, _vp, _vp, _ll, _vp, _ll, _vp, _i, _i, _i, _i, _f, _vp],
     "st2_attention_tc_supported": [_ll, _ll, _ll, _i],
     "st2_attention_tc": [_vp, _ll, _vp, _vp, _ll, _vp, _ll, _vp, _i, _i, _i, _i, _f, _vp],
+    "st2_attention_tc_packed": [_vp, _ll, _vp, _vp, _ll, _vp, _ll, _vp, _i, _i, _i, _i, _f, _vp],
     "st2_embedding_sum_rows": [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp],
     "st2_lstm_bidir": [_vp, _vp, _vp, _ll, _ll, _ll, _vp, _i, _i, _i, _vp, _vp],
     "st2_kdiff_step": [_vp, _vp, _vp, _f, _f, _f, _f, _vp, _f, _vp, _f, _vp, _i, _vp],

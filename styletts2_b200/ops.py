@@ -302,8 +302,8 @@ def channel_layernorm_lrelu(x, gamma, beta, lengths=None, eps=1e-5, slope=0.2):
 
 
 # ------------------------------------------------------------------ rows
-def rows_ln(*, B, N, Cw, h_in=None, x=None, xs=1.0, emb=None, add=None, h_out=None, g1=None, b1=None, g2=None, b2=None,
-            gb_bstride=0, ada=False, out1=None, out2=None, eps=1e-5, lengths=None):
+def _rows_args(*, B, N, Cw, h_in=None, x=None, xs=1.0, emb=None, add=None, h_out=None, g1=None, b1=None, g2=None, b2=None,
+               gb_bstride=0, ada=False, out1=None, out2=None, eps=1e-5, lengths=None):
     a = RowsArgs()
     a.h_in, a.h_in_ld = ptr(h_in), (h_in.stride(-2) if h_in is not None else 0)
     a.x, a.Cx, a.xs = ptr(x), (x.shape[-1] if x is not None else 0), xs
@@ -315,7 +315,18 @@ def rows_ln(*, B, N, Cw, h_in=None, x=None, xs=1.0, emb=None, add=None, h_out=No
     a.out2, a.out2_ld = ptr(out2), (out2.stride(-2) if out2 is not None else 0)
     a.B, a.N, a.C, a.eps = B, N, Cw, eps
     a.lengths = ptr(lengths)
-    L.call("st2_rows_ln", C.byref(a), stream_ptr())
+    return a
+
+
+def rows_ln(*, B, N, Cw, **kw):
+    L.call("st2_rows_ln", C.byref(_rows_args(B=B, N=N, Cw=Cw, **kw)), stream_ptr())
+
+
+def rows_ln_packed(*, row_utt, M, B, Cw, **kw):
+    """rows_ln over M packed token rows; row_utt (int32 [M]) gives each row's utterance, which selects x, add and the
+    per-utterance g/b rows.  No row is masked: a packed buffer holds valid rows only."""
+    with _prof(f"rows_ln_packed M{M} C{Cw} B{B}", 0.0, 4.0 * M * Cw * 3):
+        L.call("st2_rows_ln_packed", C.byref(_rows_args(B=B, N=1, Cw=Cw, **kw)), ptr(row_utt), M, stream_ptr())
 
 
 def bcast_cols(dst, col0, src, lengths=None):
@@ -329,6 +340,15 @@ def mean_rows(h, B, N):
     Cw = h.shape[-1]
     out = empty(B, Cw, device=h.device)
     L.call("st2_mean_rows", ptr(h), h.stride(-2), B, N, Cw, ptr(out), stream_ptr())
+    return out
+
+
+def mean_segments(h, offsets, B):
+    """out[b] = mean of packed rows offsets[b] .. offsets[b+1]-1 of h (offsets int32 [B+1]), in mean_rows' summation order"""
+    Cw = h.shape[-1]
+    out = empty(B, Cw, device=h.device)
+    with _prof(f"mean_segments M{h.shape[0]} C{Cw} B{B}", 0.0, 4.0 * (h.shape[0] + B) * Cw):
+        L.call("st2_mean_segments", ptr(h), h.stride(-2), ptr(offsets), B, Cw, ptr(out), stream_ptr())
     return out
 
 
@@ -429,6 +449,26 @@ def attention_ex(q, k, v, out, B, N, H, D, lengths=None):
     with _prof(f"attention{'_tc' if use_tc else ''} B{B} N{N} H{H} D{D}", 4.0 * B * H * N * N * D, 4.0 * B * N * H * D * 4, 3 if use_tc else 0):
         L.call("st2_attention_tc" if use_tc else "st2_attention_ex", ptr(q), q.stride(0), ptr(k), ptr(v), k.stride(0), ptr(out),
                out.stride(0), ptr(lengths), B, N, H, D, scale, stream_ptr())
+    return out
+
+
+def attention_packed(q, kv, offsets, B, max_len, H=8, D=64, out=None):
+    """q [M, H*D], kv [M, 2*H*D] (k | v) on packed token rows: utterance b owns rows offsets[b] .. offsets[b+1]-1
+    (offsets int32 [B+1] on the device, max_len >= every row count) and attends over its own rows only -> [M, H*D].
+    Runs the wgmma kernel; a layout it cannot take is an error."""
+    M = q.shape[0]
+    if out is None:
+        out = empty(M, H * D, device=q.device)
+    k, v = kv[:, :H * D], kv[:, H * D:]
+    scale = float(D) ** -0.5
+    ok = (k.stride(0) == v.stride(0) and bool(L.load().st2_attention_tc_supported(q.stride(0), k.stride(0), out.stride(0), D))
+          and all(t.data_ptr() % 16 == 0 for t in (q, k, v, out)))
+    if not ok:
+        raise RuntimeError("attention_packed: head_features must be 64, row strides multiples of 4 floats, pointers 16-byte aligned")
+    # the algorithmic work is sum_b n_b^2 per head; max_len * M bounds it without a host read of the offsets
+    with _prof(f"attention_tc_packed M{M} B{B} maxN{max_len} H{H} D{D}", 4.0 * H * M * max_len * D, 4.0 * M * H * D * 4, 3):
+        L.call("st2_attention_tc_packed", ptr(q), q.stride(0), ptr(k), ptr(v), k.stride(0), ptr(out), out.stride(0), ptr(offsets),
+               B, max_len, H, D, scale, stream_ptr())
     return out
 
 

@@ -44,6 +44,39 @@ def plan_equal_length_batches(lengths: Sequence[int], world: int, max_batch: int
     return plan
 
 
+def plan_token_batches(lengths: Sequence[int], world: int, max_batch: int, max_rows: int) -> List[List[List[int]]]:
+    """Serving-side plan for Synthesizer.synthesize(..., token_packing=True), whose text side runs on packed token rows and
+    so takes any mix of token counts in one batch.  Utterances are sorted by token count (longest first, ties by index)
+    and cut into batches of at most `max_batch` utterances and `max_rows` tokens in all; the batches are dealt to ranks
+    longest first (cost = the batch's token sum), each to the least loaded rank (ties to the lower rank), so that rank
+    loads end within one batch's cost of each other.  Deterministic.  Returns plan[rank] = list of batches, each a list of
+    utterance indices."""
+    assert world >= 1 and max_batch >= 1 and max_rows >= 1
+    order = sorted(range(len(lengths)), key=lambda i: (-int(lengths[i]), i))
+    batches: List[Tuple[int, List[int]]] = []
+    cur: List[int] = []
+    rows = 0
+    for i in order:
+        n = int(lengths[i])
+        if n < 1 or n > max_rows:
+            raise ValueError(f"utterance {i} has {n} tokens; a batch holds 1 .. max_rows={max_rows}")
+        if cur and (len(cur) == max_batch or rows + n > max_rows):
+            batches.append((rows, cur))
+            cur, rows = [], 0
+        cur.append(i)
+        rows += n
+    if cur:
+        batches.append((rows, cur))
+    batches.sort(key=lambda b: (-b[0], b[1][0]))
+    load = [0] * world
+    plan: List[List[List[int]]] = [[] for _ in range(world)]
+    for cost, idx in batches:
+        r = min(range(world), key=lambda q: (load[q], q))
+        plan[r].append(idx)
+        load[r] += cost
+    return plan
+
+
 def init_from_env(backend: str = "nccl"):
     """torchrun environment -> (rank, local_rank, world).  Single process if WORLD_SIZE is unset."""
     world = int(os.environ.get("WORLD_SIZE", "1"))
