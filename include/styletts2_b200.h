@@ -103,7 +103,8 @@ int st2_conv_stats_parts(int Lq);
  *   ST2_TC_F16X3     the accurate planes in a single accumulator (A/B testing).
  * `wtc` is the st2_conv_tc_weight_layout buffer (st2_conv_tc_weight_bytes bytes) built from the folded fp32 weight
  * [Cout,Cin,K] FOR THE SAME mode.  a->w is ignored; every other field means what it means for st2_conv1d,
- * except that it writes ONE statistics partial per 64-column tile (stats_nparts >= offset + ceil(Lq/64)).
+ * except that the output positions must be contiguous (y_tstride == 1, y_toffset == 0), there is no reflection
+ * duplicate (dup_q0_to < 0), and it writes ONE statistics partial per 64-column tile (stats_nparts >= offset + ceil(Lq/64)).
  * x must live in an allocation whose first byte is 16-byte aligned (cudaMalloc / the PyTorch caching allocator):
  * rows are fetched as 16-byte copies of their aligned superset window.  Operand range: |z| < 1000 after the
  * prologue, |w| < 16 (fp16 planes of 64 z and 4096 w); larger values give inf/NaN loudly.
@@ -112,32 +113,28 @@ int st2_conv_stats_parts(int Lq);
 #define ST2_TC_ACCURATE 1
 #define ST2_TC_F16X3 2
 /* Flag OR-ed into `mode` (FAST recipe, Cout <= 128): TIME-MAJOR weight layout and kernel -- frames on the MMA's M axis
- * (two M = 128 blocks per 256-frame tile), output channels on N = Cout rounded up to 32 (16 for Cout <= 16): no
- * tensor-pipe time or weight traffic for absent channels, epilogue stores straight from the accumulator registers (a warp
- * = 32 consecutive frames of one row), residual rows prefetched through a cp.async ring in shared memory, up to 8
- * accumulators in registers.  Layout and launch must use the same mode value.  Not with dup_q0_to >= 0.  (Cout = 256 as two
- * channel blocks was measured: no gain over the channel-major kernel and 3-16 % slower narrow layers from the extra tile
- * decode -- not kept.) */
+ * (each of the two consumer warpgroups takes 64 frames of a 128-frame tile), output channels on N = Cout rounded up to 32
+ * (16 for Cout <= 16): no tensor-pipe time or weight traffic for absent channels.  One fp16 and one e4m3 accumulator per
+ * warpgroup; the epilogue computes the output values through a shared-memory slot, group by group, and reduces the
+ * InstanceNorm partials over the warpgroup's four warps in shared memory.  Layout and launch must use the same mode value.
+ * (Cout = 256 as two channel blocks was measured: no gain over the channel-major kernel and 3-16 % slower narrow layers
+ * from the extra tile decode -- not kept.) */
 #define ST2_TC_TMAJOR 16
 long long st2_conv_tc_weight_bytes(int Cout, int Cin, int K);
 int st2_conv_tc_weight_layout(const float* w, void* out, int Cout, int Cin, int K, int mode, void* stream);
 int st2_conv_tc_supported(int Cin, int Cout, int K, int stride, int dil);
 int st2_conv1d_tc(const st2_conv_args* a, const void* wtc, int mode, int max_ctas, void* stream);
-/* Profiling aid: when set to a device buffer of 4*16*8 int64, CTA 0 of st2_conv1d_tc records per-role cycle
- * counters for its first 16 tiles (role 0 MMA, 1 weight producer, 2 stagers, 3 epilogue); NULL disables. */
-int st2_debug_set_trace(void* buf);
 /* Timing experiments only (tools/conv_tc_shapes.py --ablate), tensor-core convs: 4 stagers skip the conversion,
  * 16 no weight copies, 32 no raw activation copies.  Results are wrong while any bit is set; 0 restores. */
 int st2_debug_set_flags(int flags);
-/* Polyphase ConvTranspose1d on the same tensor-core kernel (one launch per phase); wtc from
- * st2_convT_tc_weight_layout (st2_convT_tc_weight_bytes bytes).  Arguments as st2_conv_transpose1d. */
+/* Polyphase ConvTranspose1d on the same tensor-core kernels (one launch per phase); wtc from
+ * st2_convT_tc_weight_layout (st2_convT_tc_weight_bytes bytes, an upper bound for every mode).  Arguments as
+ * st2_conv_transpose1d, with y rows contiguous (a->y_len = Lin*S (+1)): the S phase convolutions store contiguous rows
+ * into `tmp` (S*B*Cout*Lin floats, caller-owned), then one memory-bound kernel interleaves the phases into y, adds the
+ * residual (a->res), applies the reflection duplicate and writes ONE statistics record per (b, co) (a->stats
+ * [B,Cout,1,3], stats_nparts == 1). */
 long long st2_convT_tc_weight_bytes(int Cin, int Cout, int K, int S);
 int st2_convT_tc_weight_layout(const float* w, void* out, int Cin, int Cout, int K, int S, int P, int mode, void* stream);
-int st2_conv_transpose1d_tc(const st2_conv_args* a, const void* wtc, int mode, int K, int S, int P, int reflect_left1, void* stream);
-/* Same result through a phase-major scratch buffer: the S phase convolutions store contiguous rows into `tmp`
- * (S*B*Cout*Lin floats, caller-owned), then one memory-bound kernel interleaves the phases into y, adds the residual
- * (a->res), applies the reflection duplicate and writes ONE statistics record per (b, co) (a->stats [B,Cout,1,3],
- * stats_nparts == 1).  Strided 4-byte epilogue stores of the direct variant cost 6-10x the interleave pass. */
 int st2_conv_transpose1d_tc2(const st2_conv_args* a, const void* wtc, int mode, int K, int S, int P, int reflect_left1, float* tmp,
                              void* stream);
 
@@ -262,7 +259,7 @@ int st2_embedding_sum_rows(const long long* tokens, const float* word, const flo
  * H == 256 (every LSTM of the reference configs) runs on 8-CTA clusters with DSMEM exchange; st2_debug_lstm_cluster(0)
  * forces the cooperative-launch kernel used for other sizes (testing). */
 int st2_debug_lstm_cluster(int enable);
-/* Profiling aid (like st2_debug_set_trace): device buffer of 8 int64 <- per-phase cycle sums of CTA 0 / thread 0 of the
+/* Profiling aid: device buffer of 8 int64 <- per-phase cycle sums of CTA 0 / thread 0 of the
  * cluster LSTM kernel {wait, fma, reduce, gates, push, steps}; NULL disables. */
 int st2_debug_lstm_trace(void* buf);
 int st2_lstm_bidir(const float* gx, const float* whh, float* out, long long o_bs, long long o_ts, long long o_cs,

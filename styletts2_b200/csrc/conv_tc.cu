@@ -27,18 +27,22 @@
 //    fused into the staging) and re-used by all K taps.
 //  * Raw fp32 frame windows travel HBM -> shared memory as 16-byte cp.async copies of the ALIGNED superset window of
 //    every channel row (rows of odd length start at any 4-byte phase; the phase becomes a per-channel offset of the
-//    scalar shared-memory reads of the conversion), four blocks in flight per SM.
+//    scalar shared-memory reads of the conversion), a ring of four blocks per SM.
 //  * D accumulators live in the registers of two consumer warpgroups (output channels 0-63 / 64-127 of the tile, 128 frames
 //    each: m64n128 MMAs); the epilogue works on the fragments and fuses bias, residual, MRF accumulation and the InstanceNorm
 //    partial statistics (count, mean, M2) exactly like the SIMT kernel.  A 128-frame tile writes two partials, one per
-//    64 frames, so the statistics layout does not depend on the tile width.
+//    64 frames, so the statistics layout does not depend on the tile width.  Output positions are contiguous
+//    (y_tstride = 1, no reflection duplicate): a ConvTranspose1d runs its phases into phase-major scratch rows that
+//    convT_interleave_kernel interleaves (st2_conv_transpose1d_tc2).
 //  * Warp roles in whole warpgroups: warps 0-7 = consumers (wgmma + epilogue), warp 8 = weight TMA producer, warps 9-14 =
 //    activation stagers, warp 15 idle.  setmaxnreg moves registers from warpgroups 2-3 to the consumers (arithmetic at
 //    THREADS below).  Persistent CTAs (one per SM) loop over tiles.
 //
-// TWO kernels share the stager and weight-producer roles (device functions below): the channel-major conv1d_tc_kernel
-// described above and the TIME-MAJOR conv1d_tct_kernel further down (FAST recipe, Cout <= 128: frames on the MMA's M axis,
-// output channels on N; its header comment has the mapping).
+// TWO kernels share this pipeline (barriers, producer roles and the consumer K-loop, device functions below): the
+// channel-major conv1d_tc_kernel described above and the TIME-MAJOR conv1d_tct_kernel further down (FAST recipe,
+// Cout <= 128: frames on the MMA's M axis, output channels on N; its header comment has the mapping).  They differ in the
+// MMAs of one tap, the taps per weight stage and their epilogues.  One layout kernel writes the weight blocks of both, for
+// a conv and for the phases of a ConvTranspose1d.
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
 
@@ -101,7 +105,7 @@ constexpr float F8_WLO = 16.0f, F8_WHI = 1.0f / 256.0f, F8_XHI = 1.0f / 16.0f, F
 
 // Range guard (as in linear_tc.cu, with a flag of its own): the fp16 high planes hold |z'| = 64 |z| and |w'| = 4096 |w| below
 // 65504, i.e. |z| < 1023.5 after the prologue and |w| < 16; beyond that (or for NaN) the conv writes inf/NaN.  Every stager
-// thread keeps one predicate over the rows it converts and raises the flag once; the weight layout kernels check the weights.
+// thread keeps one predicate over the rows it converts and raises the flag once; the weight layout kernel checks the weights.
 // st2_range_flag_fetch() reports and clears it.  Not covered: the FAST recipe's e4m3 corrections saturate (silently, to
 // +-448) from |z| of about 64 on (DESIGN.md "Precision recipes").
 __device__ int g_range_flag = 0;
@@ -132,7 +136,6 @@ static_assert(8 * B_COUNT + 8 <= 512, "barrier area");
 // Timing-experiment switches (tools/conv_tc_shapes.py --ablate; results are WRONG when any is set; 0 in production):
 //   4 = stagers skip the conversion (stale operands), 16 = no weight copies, 32 = no raw activation copies
 __device__ int g_dbg = 0;
-__device__ long long* g_trace = nullptr;   // reserved for per-role cycle traces (st2_debug_set_trace); unused by these kernels
 
 using namespace st2::ptx;
 
@@ -415,6 +418,87 @@ __device__ __forceinline__ void release(const uint32_t bar0, const Pending& p, c
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// Pipeline skeleton of both kernels: barriers, producer roles and the consumer K-loop.  The kernels differ only in the
+// MMAs of one tap, the taps per weight stage and their epilogues.
+__device__ __forceinline__ void init_barriers(const uint32_t bar0) {
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < W_STAGES; ++i) { mbar_init(bar0 + 8u * (B_WFULL + i), 1); mbar_init(bar0 + 8u * (B_WEMPTY + i), 2); }
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(bar0 + 8u * (B_AFULL + i), NUM_STAGERS);
+      mbar_init(bar0 + 8u * (B_AEMPTY + i), 2);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+}
+
+// Warpgroups 2-3: give registers back, then run the weight producer (warp 8, one lane) or an activation stager.
+template <int MODE>
+__device__ __forceinline__ void producer_roles(const st2_conv_args& a, const uint4* __restrict__ wtc, uint8_t* smem, const int ncb,
+                                               const int RW, const int wstep, const int tps, const int stage_bytes, const int ntiles,
+                                               const int n_tq, const int n_cob, const int tid, const int warp, const int lane) {
+  const uint32_t sbase = smem_u32(smem), bar0 = sbase + SM_BAR;
+  reg_dealloc<REG_AUX>();
+  if (warp == NUM_CONS / 32) {
+    if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, a.K, wstep, tps, stage_bytes, ntiles, n_tq, n_cob);
+  } else if (warp < (ST0 + NUM_STAGERS) / 32) {
+    stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
+  }
+}
+
+// Ring positions of a consumer warpgroup and its wgmma group still in flight, carried from tile to tile.
+struct ConsumerRing {
+  int ws = 0, wph = 0, as = 0, aph = 0;
+  Pending pend{-1, -1};
+};
+
+// Consumer K-loop of one tile: per 16-channel block wait for the staged window, then per weight stage of up to `tps` taps
+// wait for the weights and issue the stage's MMAs as one wgmma group; the previous group's stage is released once the wait
+// leaves this one pending.  mma(w_addr, x_addr, acc) issues one tap: its weights at w_addr (+ w_off in the stage, wstep
+// bytes per tap), its window at x_addr (+ x_off in the buffer, one dilation per tap).  TPS > 0 unrolls a compile-time tps.
+// Returns with every MMA complete and every stage released; the caller fences its accumulators (wg_fence_regs).
+template <int TPS, class Mma>
+__device__ __forceinline__ void consumer_k_loop(ConsumerRing& r, const uint32_t sbase, const bool leader, const int ncb, const int K,
+                                                const int tps, const int stage_bytes, const int wstep, const uint32_t w_off,
+                                                const uint32_t x_off, const uint32_t dil16, Mma&& mma) {
+  const uint32_t bar0 = sbase + SM_BAR;
+  uint32_t acc = 0;
+  for (int cb = 0; cb < ncb; ++cb) {
+    mbar_wait(bar0 + 8u * (B_AFULL + r.as), r.aph);
+    uint32_t x_addr = sbase + SM_ACT + r.as * ACT_BUF_BYTES + x_off;
+    for (int tap0 = 0; tap0 < K; tap0 += tps) {
+      mbar_wait(bar0 + 8u * (B_WFULL + r.ws), r.wph);
+      wg_fence();
+      uint32_t w_addr = sbase + SM_W + r.ws * stage_bytes + w_off;
+      const int nt = min(tps, K - tap0);
+      auto tap = [&] {
+        mma(w_addr, x_addr, acc);
+        acc = 1;
+        w_addr += wstep;
+        x_addr += dil16;
+      };
+      if constexpr (TPS > 0) {
+#pragma unroll
+        for (int t = 0; t < TPS; ++t)
+          if (t < nt) tap();
+      } else {
+        for (int t = 0; t < nt; ++t) tap();
+      }
+      wg_commit();
+      wg_wait<1>();
+      release(bar0, r.pend, leader);
+      r.pend.ws = r.ws;
+      r.pend.as = (tap0 + tps >= K) ? r.as : -1;
+      if (++r.ws == W_STAGES) { r.ws = 0; r.wph ^= 1; }
+    }
+    if (++r.as == 2) { r.as = 0; r.aph ^= 1; }
+  }
+  wg_wait<0>();
+  release(bar0, r.pend, leader);
+  r.pend.ws = -1;
+}
+
 // Output value of one element: bias, residual, divisor, MRF accumulation and output activation, in the order of the SIMT
 // kernel.  res_v = the residual, y_old = the y value the MRF accumulation adds to (each read only when its mode is on).
 __device__ __forceinline__ float epi_combine(const st2_conv_args& a, float v, float bias, float res_v, float y_old) {
@@ -437,15 +521,6 @@ __device__ __forceinline__ void epi_load(const st2_conv_args& a, const float* rr
   y_old = (a.accum_mode != 0 && ok) ? yp[oidx] : 0.f;
 }
 
-// One element, loads and store together (the reflection duplicate, one element per row).  Returns the value written.
-__device__ __forceinline__ float epi_value(const st2_conv_args& a, float v, float bias, const float* rrow, float* yp, int oidx) {
-  float res_v, y_old;
-  epi_load(a, rrow, yp, oidx, true, res_v, y_old);
-  const float val = epi_combine(a, v, bias, res_v, y_old);
-  yp[oidx] = val;
-  return val;
-}
-
 template <int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
 conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int ncb, const int RW, const int ntiles,
@@ -455,19 +530,7 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = warp_uniform(tid), lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = sbase + SM_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-
-  if (tid == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(BAR(B_AFULL + i), NUM_STAGERS);
-      mbar_init(BAR(B_AEMPTY + i), 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  const int K = a.K;
+  init_barriers(sbase + SM_BAR);
 
   if (warp < NUM_CONS / 32) {
     // ================================================================ consumers: wgmma (warpgroup wg = channels 64 wg ..) + epilogue
@@ -475,59 +538,31 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
     const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
     const bool leader = (tid & 127) == 0;
     const uint32_t lbo_a = TM * 16, lbo_b = (uint32_t)RWP * 16;
-    const uint32_t dil16 = (uint32_t)a.dil * 16u;
-    int ws = 0, wph = 0, as = 0, aph = 0;
-    Pending pend{-1, -1};
+    ConsumerRing ring;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const TileCoord tc_ = tile_coord(tile, n_tq, n_cob);
       float d0[64], d1[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
-      uint32_t acc = 0;
-      for (int cb = 0; cb < ncb; ++cb) {
-        mbar_wait(BAR(B_AFULL + as), aph);
-        uint32_t b_addr = sbase + SM_ACT + as * ACT_BUF_BYTES;
-        for (int tap0 = 0; tap0 < K; tap0 += TPS) {
-          mbar_wait(BAR(B_WFULL + ws), wph);
-          wg_fence();
-          uint32_t a_addr = sbase + SM_W + ws * W_STAGE_BYTES + wg * 64 * 16;
-          const int nt = min(TPS, K - tap0);
-#pragma unroll
-          for (int t = 0; t < TPS; ++t) {
-            if (t < nt) {
-              const uint64_t da0 = make_desc(a_addr, lbo_a, 128), da1 = make_desc(a_addr + W_PLANE_BYTES, lbo_a, 128);
-              const uint64_t db0 = make_desc(b_addr, lbo_b, 128), db1 = make_desc(b_addr + ACT_PLANE_BYTES, lbo_b, 128);
-              if (MODE == MODE_FAST) {
-                wgmma_f16_n128(d0, da0, db0, acc);
-                wgmma_e4m3_n128(d1, da1, db1, acc);     // both corrections in one e4m3 K=32 MMA, own accumulator
-              } else if (MODE == MODE_ACC) {
-                wgmma_f16_n128(d0, da0, db0, acc);
-                wgmma_f16_n128(d1, da0, db1, acc);
-                wgmma_f16_n128(d1, da1, db0, 1u);
-              } else {
-                wgmma_f16_n128(d0, da0, db0, acc);
-                wgmma_f16_n128(d0, da0, db1, 1u);
-                wgmma_f16_n128(d0, da1, db0, 1u);
-              }
-              acc = 1;
-              a_addr += W_STEP_BYTES;
-              b_addr += dil16;
-            }
-          }
-          wg_commit();
-          wg_wait<1>();
-          release(bar0, pend, leader);
-          pend.ws = ws;
-          pend.as = (tap0 + TPS >= K) ? as : -1;
-          if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
+      consumer_k_loop<TPS>(ring, sbase, leader, ncb, a.K, TPS, W_STAGE_BYTES, W_STEP_BYTES, wg * 64 * 16, 0, (uint32_t)a.dil * 16u,
+                           [&](uint32_t a_addr, uint32_t b_addr, uint32_t acc) {
+        const uint64_t da0 = make_desc(a_addr, lbo_a, 128), da1 = make_desc(a_addr + W_PLANE_BYTES, lbo_a, 128);
+        const uint64_t db0 = make_desc(b_addr, lbo_b, 128), db1 = make_desc(b_addr + ACT_PLANE_BYTES, lbo_b, 128);
+        if (MODE == MODE_FAST) {
+          wgmma_f16_n128(d0, da0, db0, acc);
+          wgmma_e4m3_n128(d1, da1, db1, acc);     // both corrections in one e4m3 K=32 MMA, own accumulator
+        } else if (MODE == MODE_ACC) {
+          wgmma_f16_n128(d0, da0, db0, acc);
+          wgmma_f16_n128(d1, da0, db1, acc);
+          wgmma_f16_n128(d1, da1, db0, 1u);
+        } else {
+          wgmma_f16_n128(d0, da0, db0, acc);
+          wgmma_f16_n128(d0, da0, db1, 1u);
+          wgmma_f16_n128(d0, da1, db0, 1u);
         }
-        if (++as == 2) { as = 0; aph ^= 1; }
-      }
-      wg_wait<0>();
+      });
       wg_fence_regs(d0);
       if (MODE != MODE_X3) wg_fence_regs(d1);
-      release(bar0, pend, leader);
-      pend.ws = -1;
       // fold the correction accumulator: d0 holds the unscaled sums from here on (d1 is dead)
 #pragma unroll
       for (int r = 0; r < 64; ++r) {
@@ -567,7 +602,7 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
 #pragma unroll
               for (int c = 0; c < 2; ++c) {
                 const int col = 8 * (j0 + jj) + 2 * t4 + c;
-                epi_load(a, rrow, yp, (t0 + col) * a.y_tstride + a.y_toffset, cok && col < ncols, res_v[2 * jj + c], y_old[2 * jj + c]);
+                epi_load(a, rrow, yp, t0 + col, cok && col < ncols, res_v[2 * jj + c], y_old[2 * jj + c]);
               }
             }
 #pragma unroll
@@ -576,21 +611,14 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
               for (int c = 0; c < 2; ++c) {
                 const int j = j0 + jj;
                 const int r = 4 * (8 * h + j) + 2 * i + c, col = 8 * j + 2 * t4 + c;
-                const float v = d0[r];
                 float val = 0.f;
                 if (cok && col < ncols) {
-                  val = epi_combine(a, v, bias, res_v[2 * jj + c], y_old[2 * jj + c]);
-                  yp[(t0 + col) * a.y_tstride + a.y_toffset] = val;
+                  val = epi_combine(a, d0[r], bias, res_v[2 * jj + c], y_old[2 * jj + c]);
+                  yp[t0 + col] = val;
                   s += val;
                   n += 1.f;
                 }
                 d0[r] = val;
-                // ReflectionPad1d((1,0)) duplicate of the q==0 column (istftnet.py:365-366): value differs by its residual
-                if (col == 0 && t0 == 0 && a.dup_q0_to >= 0 && cok) {
-                  const float dv = epi_value(a, v, bias, rrow, yp, a.dup_q0_to);
-                  s += dv;   // one extra sample of this row
-                  n += 1.f;
-                }
               }
             }
           }
@@ -611,10 +639,6 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
                 if (col < ncols) m2 = fmaf(dv, dv, m2);
               }
             }
-            if (t0 == 0 && a.dup_q0_to >= 0 && t4 == 0 && cok) {
-              const float dv = yp[a.dup_q0_to] - mean;
-              m2 = fmaf(dv, dv, m2);
-            }
             m2 += __shfl_xor_sync(0xffffffffu, m2, 1);
             m2 += __shfl_xor_sync(0xffffffffu, m2, 2);
             if (t4 == 0 && cok) {
@@ -627,13 +651,7 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
       }
     }
   } else {
-    reg_dealloc<REG_AUX>();
-    if (warp == NUM_CONS / 32) {
-      // ================================================================ weight producer (1-D TMA bulk copies)
-      if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, W_STEP_BYTES, TPS, W_STAGE_BYTES, ntiles, n_tq, n_cob);
-    } else if (warp < (ST0 + NUM_STAGERS) / 32) {
-      stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, n_cob, tid, warp, lane);
-    }
+    producer_roles<MODE>(a, wtc, smem, ncb, RW, W_STEP_BYTES, TPS, W_STAGE_BYTES, ntiles, n_tq, n_cob, tid, warp, lane);
   }
 }
 
@@ -673,19 +691,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
   extern __shared__ __align__(1024) uint8_t smem[];
   const int tid = threadIdx.x, warp = warp_uniform(tid), lane = tid & 31;
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = sbase + SM_BAR;
-  auto BAR = [&](int i) { return bar0 + 8u * i; };
-
-  if (tid == 0) {
-    for (int i = 0; i < W_STAGES; ++i) { mbar_init(BAR(B_WFULL + i), 1); mbar_init(BAR(B_WEMPTY + i), 2); }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(BAR(B_AFULL + i), NUM_STAGERS);
-      mbar_init(BAR(B_AEMPTY + i), 2);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  const int K = a.K;
+  init_barriers(sbase + SM_BAR);
   const int wstep = 64 * NC;                      // bytes of one (16 channels, tap) step: 2 planes x 2 chunks x NC rows x 16 B
   const int tps = T_WSTAGE / wstep;               // taps per weight stage: 1 (NC = 128, 96) .. 8 (NC = 16)
 
@@ -694,48 +700,24 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
     const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t4 = lane & 3;
     const bool leader = (tid & 127) == 0;
     const uint32_t lbo_x = (uint32_t)RWP * 16, lbo_w = (uint32_t)NC * 16;
-    const uint32_t dil16 = (uint32_t)a.dil * 16u;
     float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * TCT_NC_MAX;   // [4 warps][TCT_NC_MAX channels]
     float4* slot = reinterpret_cast<float4*>(smem + SM_SLOT) + tid;              // this thread's float4 q at slot[q * NUM_CONS]
-    int ws = 0, wph = 0, as = 0, aph = 0;
-    Pending pend{-1, -1};
+    ConsumerRing ring;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int tq = tile % n_tq, b = tile / n_tq;
       float d[NC / 2], e[NC / 2];   // fp16 main products / e4m3 correction products (e4m3 wgmma accumulates at reduced precision)
 #pragma unroll
       for (int i = 0; i < NC / 2; ++i) { d[i] = 0.f; e[i] = 0.f; }
-      uint32_t acc = 0;
-      for (int cb = 0; cb < ncb; ++cb) {
-        mbar_wait(BAR(B_AFULL + as), aph);
-        uint32_t x_addr = sbase + SM_ACT + as * ACT_BUF_BYTES + wg * TP * 16;   // warpgroup wg: frames TP wg .. of the tile
-        for (int tap0 = 0; tap0 < K; tap0 += tps) {
-          mbar_wait(BAR(B_WFULL + ws), wph);
-          wg_fence();
-          const int nt = min(tps, K - tap0);
-          uint32_t w_addr = sbase + SM_W + ws * T_WSTAGE;
-          for (int t = 0; t < nt; ++t) {
-            tct_mma<NC>(d, e, make_desc(x_addr, lbo_x, 128), make_desc(w_addr, lbo_w, 128), make_desc(x_addr + ACT_PLANE_BYTES, lbo_x, 128),
-                        make_desc(w_addr + 2 * NC * 16, lbo_w, 128), acc);
-            acc = 1;
-            w_addr += wstep;
-            x_addr += dil16;
-          }
-          wg_commit();
-          wg_wait<1>();
-          release(bar0, pend, leader);
-          pend.ws = ws;
-          pend.as = (tap0 + tps >= K) ? as : -1;
-          if (++ws == W_STAGES) { ws = 0; wph ^= 1; }
-        }
-        if (++as == 2) { as = 0; aph ^= 1; }
-      }
-      wg_wait<0>();
+      // warpgroup wg: frames TP wg .. of the tile
+      consumer_k_loop<0>(ring, sbase, leader, ncb, a.K, tps, T_WSTAGE, wstep, 0, wg * TP * 16, (uint32_t)a.dil * 16u,
+                         [&](uint32_t w_addr, uint32_t x_addr, uint32_t acc) {
+        tct_mma<NC>(d, e, make_desc(x_addr, lbo_x, 128), make_desc(w_addr, lbo_w, 128), make_desc(x_addr + ACT_PLANE_BYTES, lbo_x, 128),
+                    make_desc(w_addr + 2 * NC * 16, lbo_w, 128), acc);
+      });
       wg_fence_regs(d);
       wg_fence_regs(e);
 #pragma unroll
       for (int i = 0; i < NC / 2; ++i) d[i] += e[i];
-      release(bar0, pend, leader);
-      pend.ws = -1;
 
       // ---- epilogue: row = frame, column = output channel.  The warpgroup's 64 frames are one statistics partial; the
       // second warpgroup of a tail tile can lie entirely beyond Lq (ncols <= 0): it then writes nothing.
@@ -755,7 +737,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
 #pragma unroll
           for (int i = 0; i < 2; ++i) {
             const int fr = w * 16 + g + 8 * i;
-            epi_load(a, rrow, yp, (t0 + fr) * a.y_tstride + a.y_toffset, cok && fr < ncols, res_n[2 * i + c], old_n[2 * i + c]);
+            epi_load(a, rrow, yp, t0 + fr, cok && fr < ncols, res_n[2 * i + c], old_n[2 * i + c]);
           }
         }
       };
@@ -790,7 +772,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
               float val = 0.f;
               if (cok && fr < ncols) {
                 val = epi_combine(a, v[2 * i + c] * D_UNSCALE, bias, res_v[2 * i + c], y_old[2 * i + c]);
-                yp[(t0 + fr) * a.y_tstride + a.y_toffset] = val;
+                yp[t0 + fr] = val;
               }
               o[2 * i + c] = val;
             }
@@ -894,13 +876,7 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
       }
     }
   } else {
-    reg_dealloc<REG_AUX>();
-    if (warp == NUM_CONS / 32) {
-      // ================================================================ weight producer (1-D TMA bulk copies)
-      if (lane == 0) weight_producer_role(wtc, sbase, bar0, ncb, K, wstep, tps, T_WSTAGE, ntiles, n_tq, 1);
-    } else if (warp < (ST0 + NUM_STAGERS) / 32) {
-      stager_role<MODE>(a, smem, sbase, bar0, ncb, RW, ntiles, n_tq, 1, tid, warp, lane);
-    }
+    producer_roles<MODE>(a, wtc, smem, ncb, RW, wstep, tps, T_WSTAGE, ntiles, n_tq, 1, tid, warp, lane);
   }
 }
 
@@ -945,11 +921,15 @@ __device__ __forceinline__ int weight_row_channel(int Cout, int cob, int col, bo
   return co < Cout ? co : -1;
 }
 
-// fp32 [Cout,Cin,K] -> step blocks [n_cob][ncb][K] x (64 * rows) bytes (the taps of one 16-channel block are contiguous)
-__global__ void conv_tc_weight_layout_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int Cout, int Cin, int K,
-                                             int n_cob, int ncb, int mode, int rows, int tmajor) {
-  // one thread per (stage, plane, chunk, row): writes the 16 bytes of that row
-  const long long total = (long long)K * n_cob * ncb * 2 * KCB * rows;
+// fp32 weights -> S phases of step blocks [n_cob][ncb][J] x (64 * rows) bytes, phase_bytes apart (the taps of one 16-channel
+// block are contiguous).  Tap kp of phase ph reads source tap k = k0 + (ph + P) % S + kp * k_step of element (co, ci) at
+// w[co * co_stride + ci * ci_stride + k]; k >= K reads zero.  A conv is S = 1, k0 = 0, k_step = 1; a ConvTranspose1d phase
+// (a J-tap stride-1 conv, see conv.cu) reads its taps backwards, k0 = (J - 1) S, k_step = -S.
+__global__ void weight_layout_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int Cout, int Cin, int K, long long co_stride,
+                                     long long ci_stride, int S, int P, int J, int k0, int k_step, long long phase_bytes, int n_cob, int ncb,
+                                     int mode, int rows, int tmajor) {
+  // one thread per (phase, stage, plane, chunk, row): writes the 16 bytes of that row
+  const long long total = (long long)S * J * n_cob * ncb * 2 * KCB * rows;
   const int step_bytes = 2 * KCB * rows * 16;
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     long long r = i;
@@ -958,47 +938,18 @@ __global__ void conv_tc_weight_layout_kernel(const float* __restrict__ w, uint8_
     const int plane = (int)(r % 2); r /= 2;
     const int cb = (int)(r % ncb); r /= ncb;
     const int cob = (int)(r % n_cob); r /= n_cob;
-    const int tap = (int)r;
+    const int kp = (int)(r % J);
+    const int ph = (int)(r / J);
     const int co = weight_row_channel(Cout, cob, col, tmajor != 0);
+    const int k = k0 + (ph + P) % S + kp * k_step;
     float wr[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
       const int ci = cb * CB + j;
-      wr[j] = (co >= 0 && ci < Cin) ? w[((long long)co * Cin + ci) * K + tap] : 0.f;
+      wr[j] = (co >= 0 && ci < Cin && k < K) ? w[co * co_stride + ci * ci_stride + k] : 0.f;
     }
     weight_range_note(wr);
-    uint8_t* blk = out + (((long long)cob * ncb + cb) * K + tap) * step_bytes;
-    const int base = plane * (KCB * rows * 16) + (chunk * rows + col) * 16;
-#pragma unroll
-    for (int b = 0; b < 16; ++b) weight_stage_store(blk, base + b, mode, wr, rows);
-  }
-}
-
-// ConvTranspose1d weight [Cin,Cout,K] -> S per-phase tensor-core blocks (phase r = J-tap stride-1 conv, see conv.cu)
-__global__ void convT_tc_weight_layout_kernel(const float* __restrict__ w, uint8_t* __restrict__ out, int Cin, int Cout, int K,
-                                              int S, int P, int J, int n_cob, int ncb, int mode, int rows, int tmajor) {
-  const long long per_phase = (long long)J * n_cob * ncb * 2 * KCB * rows;
-  const long long total = per_phase * S;
-  const int step_bytes = 2 * KCB * rows * 16;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const int ph = (int)(i / per_phase);
-    long long r = i % per_phase;
-    const int col = (int)(r % rows); r /= rows;
-    const int chunk = (int)(r % KCB); r /= KCB;
-    const int plane = (int)(r % 2); r /= 2;
-    const int cb = (int)(r % ncb); r /= ncb;
-    const int cob = (int)(r % n_cob); r /= n_cob;
-    const int kp = (int)r;  // tap of the phase conv
-    const int co = weight_row_channel(Cout, cob, col, tmajor != 0);
-    const int kk = (J - 1 - kp) * S + ((ph + P) % S);
-    float wr[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const int ci = cb * CB + j;
-      wr[j] = (co >= 0 && ci < Cin && kk < K) ? w[((long long)ci * Cout + co) * K + kk] : 0.f;
-    }
-    weight_range_note(wr);
-    uint8_t* blk = out + ((long long)ph * J * n_cob * ncb + ((long long)cob * ncb + cb) * J + kp) * step_bytes;
+    uint8_t* blk = out + ph * phase_bytes + (((long long)cob * ncb + cb) * J + kp) * step_bytes;
     const int base = plane * (KCB * rows * 16) + (chunk * rows + col) * 16;
 #pragma unroll
     for (int b = 0; b < 16; ++b) weight_stage_store(blk, base + b, mode, wr, rows);
@@ -1075,17 +1026,25 @@ static long long weight_bytes_mode(int Cout, int Cin, int K, int mode) {
   return (long long)K * cdiv(Cout, TM) * ncb * W_STEP_BYTES;
 }
 
+// Layout of S phases of J taps (see weight_layout_kernel), each phase weight_bytes_mode(Cout, Cin, J, mode) bytes.
+static void weight_layout(const float* w, void* out, int Cout, int Cin, int K, long long co_stride, long long ci_stride, int S, int P,
+                          int J, int k0, int k_step, int mode, cudaStream_t st) {
+  const bool tm = (mode & TMAJOR) != 0;
+  const int n_cob = tm ? 1 : cdiv(Cout, TM), ncb = cdiv(Cin, CB), rows = tm ? tmajor_nc(Cout) : TM;
+  weight_layout_kernel<<<1024, 256, 0, st>>>(w, (uint8_t*)out, Cout, Cin, K, co_stride, ci_stride, S, P, J, k0, k_step,
+                                             weight_bytes_mode(Cout, Cin, J, mode), n_cob, ncb, mode & ~TMAJOR, rows, tm ? 1 : 0);
+  ++g_launches;
+}
+
 static int launch_tc(const st2_conv_args& a, const void* wtc, int mode, int max_ctas, cudaStream_t st) {
   const bool tmajor = (mode & TMAJOR) != 0;
   const int n_tq = cdiv(a.Lq, TN), n_cob = tmajor ? 1 : cdiv(a.Cout, TM), ncb = cdiv(a.Cin, CB);
   const int rw = (TN + (a.K - 1) * a.dil + 7) & ~7;
   const int ntiles = a.B * n_cob * n_tq;
-  static int num_sms[64] = {0};   // per device ordinal (cudaFuncSetAttribute is per device too)
-  int dev = 0;
-  cudaGetDevice(&dev);
-  dev &= 63;
-  if (!num_sms[dev]) {
-    cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
+  static PerDevice once;   // cudaFuncSetAttribute is per device
+  if (once.first()) {
+    const int dev = once.dev();
+    cudaDeviceGetAttribute(&once.value[dev], cudaDevAttrMultiProcessorCount, dev);
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_FAST>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_ACC>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     cudaFuncSetAttribute(conv1d_tc_kernel<MODE_X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
@@ -1095,7 +1054,8 @@ static int launch_tc(const st2_conv_args& a, const void* wtc, int mode, int max_
     cudaFuncSetAttribute(conv1d_tct_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
     cudaFuncSetAttribute(conv1d_tct_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM_TOTAL);
   }
-  int grid = ntiles < num_sms[dev] ? ntiles : num_sms[dev];
+  const int num_sms = once.value[once.dev()];
+  int grid = ntiles < num_sms ? ntiles : num_sms;
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
   if (tmajor) {
     const int nh = tmajor_nc(a.Cout) / 2;
@@ -1143,11 +1103,8 @@ static bool tc_mode_ok(int mode, int Cout) {
 
 int st2_conv_tc_weight_layout(const float* w, void* out, int Cout, int Cin, int K, int mode, void* stream) {
   ST2_REQUIRE(w && out && Cout > 0 && Cin > 0 && K > 0 && tc_mode_ok(mode, Cout), "st2_conv_tc_weight_layout", "bad args");
-  const bool tm = (mode & tc::TMAJOR) != 0;
-  const int n_cob = tm ? 1 : cdiv(Cout, tc::TM), ncb = cdiv(Cin, tc::CB), rows = tm ? tc::tmajor_nc(Cout) : tc::TM;
-  tc::conv_tc_weight_layout_kernel<<<1024, 256, 0, (cudaStream_t)stream>>>(w, (uint8_t*)out, Cout, Cin, K, n_cob, ncb, mode & ~tc::TMAJOR,
-                                                                             rows, tm ? 1 : 0);
-  ++g_launches;
+  // w [Cout, Cin, K]: one phase, taps in order
+  tc::weight_layout(w, out, Cout, Cin, K, (long long)Cin * K, K, 1, 0, K, 0, 1, mode, (cudaStream_t)stream);
   ST2_CHECK_LAUNCH("st2_conv_tc_weight_layout");
   return 0;
 }
@@ -1161,7 +1118,8 @@ int st2_conv1d_tc(const st2_conv_args* a, const void* wtc, int mode, int max_cta
   ST2_REQUIRE(a && a->x && wtc && a->y && tc_mode_ok(mode, a->Cout), "st2_conv1d_tc", "null pointer / bad mode");
   ST2_REQUIRE(st2_conv_tc_supported(a->Cin, a->Cout, a->K, a->stride, a->dil), "st2_conv1d_tc", "unsupported shape");
   ST2_REQUIRE(a->pre_act != ST2_ACT_SNAKE || a->pre_alpha, "st2_conv1d_tc", "snake prologue needs alpha");
-  ST2_REQUIRE(!(mode & tc::TMAJOR) || a->dup_q0_to < 0, "st2_conv1d_tc", "time-major kernel: no reflection duplicate");
+  ST2_REQUIRE(a->y_tstride == 1 && a->y_toffset == 0, "st2_conv1d_tc", "output positions must be contiguous (y_tstride 1, y_toffset 0)");
+  ST2_REQUIRE(a->dup_q0_to < 0, "st2_conv1d_tc", "no reflection duplicate (dup_q0_to < 0)");
   const int nparts = cdiv(a->Lq, tc::TP);
   ST2_REQUIRE(!a->stats || a->stats_nparts >= a->stats_part_offset + nparts, "st2_conv1d_tc", "stats buffer too small (one partial per 64 columns)");
   tc::launch_tc(*a, wtc, mode, max_ctas, (cudaStream_t)stream);
@@ -1175,13 +1133,6 @@ int st2_debug_set_flags(int flags) {
   return 0;
 }
 
-int st2_debug_set_trace(void* buf) {
-  long long* p = (long long*)buf;
-  cudaError_t e = cudaMemcpyToSymbol(tc::g_trace, &p, sizeof(p));
-  if (e != cudaSuccess) { set_error("st2_debug_set_trace", e); return (int)e; }
-  return 0;
-}
-
 long long st2_convT_tc_weight_bytes(int Cin, int Cout, int K, int S) {
   const int J = (K + S - 1) / S;
   return (long long)S * st2_conv_tc_weight_bytes(Cout, Cin, J);
@@ -1190,44 +1141,14 @@ long long st2_convT_tc_weight_bytes(int Cin, int Cout, int K, int S) {
 int st2_convT_tc_weight_layout(const float* w, void* out, int Cin, int Cout, int K, int S, int P, int mode, void* stream) {
   ST2_REQUIRE(w && out && Cout > 0 && Cin > 0 && K > 0 && S > 0 && tc_mode_ok(mode, Cout), "st2_convT_tc_weight_layout", "bad args");
   const int J = (K + S - 1) / S;
-  const bool tm = (mode & tc::TMAJOR) != 0;
-  const int n_cob = tm ? 1 : cdiv(Cout, tc::TM), ncb = cdiv(Cin, tc::CB), rows = tm ? tc::tmajor_nc(Cout) : tc::TM;
-  tc::convT_tc_weight_layout_kernel<<<1024, 256, 0, (cudaStream_t)stream>>>(w, (uint8_t*)out, Cin, Cout, K, S, P, J, n_cob, ncb,
-                                                                              mode & ~tc::TMAJOR, rows, tm ? 1 : 0);
-  ++g_launches;
+  // w [Cin, Cout, K]: phase ph = J taps read backwards from (J - 1) S + (ph + P) % S
+  tc::weight_layout(w, out, Cout, Cin, K, K, (long long)Cout * K, S, P, J, (J - 1) * S, -S, mode, (cudaStream_t)stream);
   ST2_CHECK_LAUNCH("st2_convT_tc_weight_layout");
   return 0;
 }
 
-int st2_conv_transpose1d_tc(const st2_conv_args* a0, const void* wtc, int mode, int K, int S, int P, int reflect_left1, void* stream) {
-  ST2_REQUIRE(a0 && a0->x && wtc && a0->y && tc_mode_ok(mode, a0->Cout) && !(mode & tc::TMAJOR), "st2_conv_transpose1d_tc", "null pointer / bad mode");
-  ST2_REQUIRE(K > 0 && S > 0 && P >= 0, "st2_conv_transpose1d_tc", "bad shape");
-  const int J = (K + S - 1) / S;
-  ST2_REQUIRE(st2_conv_tc_supported(a0->Cin, a0->Cout, J, 1, 1), "st2_conv_transpose1d_tc", "unsupported shape");
-  const int parts = cdiv(a0->Lin, tc::TP);
-  ST2_REQUIRE(!a0->stats || a0->stats_nparts >= S * parts, "st2_conv_transpose1d_tc", "stats buffer too small");
-  const long long phase_bytes = st2_conv_tc_weight_bytes(a0->Cout, a0->Cin, J);
-  for (int r = 0; r < S; ++r) {
-    st2_conv_args a = *a0;
-    const int cr = (r + P) / S;
-    a.K = J;
-    a.stride = 1;
-    a.dil = 1;
-    a.pad = (J - 1) - cr;
-    a.Lq = a0->Lin;
-    a.y_tstride = S;
-    a.y_toffset = r + (reflect_left1 ? 1 : 0);
-    a.y_len = a0->Lin * S + (reflect_left1 ? 1 : 0);
-    a.stats_part_offset = r * parts;
-    a.dup_q0_to = (reflect_left1 && r == 1) ? 0 : -1;
-    tc::launch_tc(a, (const uint8_t*)wtc + (size_t)r * phase_bytes, mode, 0, (cudaStream_t)stream);
-  }
-  ST2_CHECK_LAUNCH("st2_conv_transpose1d_tc");
-  return 0;
-}
-
-/* Phase-major variant: every phase writes contiguous rows into `tmp` ([S][B][Cout][Lin] floats), one memory-bound pass
- * interleaves, adds the residual and produces ONE statistics record per row (stats [B,Cout,1,3]). */
+/* Every phase writes contiguous rows into `tmp` ([S][B][Cout][Lin] floats), one memory-bound pass interleaves, adds the
+ * residual and produces ONE statistics record per row (stats [B,Cout,1,3]). */
 int st2_conv_transpose1d_tc2(const st2_conv_args* a0, const void* wtc, int mode, int K, int S, int P, int reflect_left1, float* tmp,
                              void* stream) {
   ST2_REQUIRE(a0 && a0->x && wtc && a0->y && tmp && tc_mode_ok(mode, a0->Cout), "st2_conv_transpose1d_tc2", "null pointer / bad mode");

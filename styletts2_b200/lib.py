@@ -71,11 +71,9 @@ SIGNATURES = {
     "st2_conv_tc_weight_layout": [_vp, _vp, _i, _i, _i, _i, _vp],
     "st2_conv_tc_supported": [_i, _i, _i, _i, _i],
     "st2_conv1d_tc": [C.POINTER(ConvArgs), _vp, _i, _i, _vp],
-    "st2_debug_set_trace": [_vp],
     "st2_debug_set_flags": [_i],
     "st2_convT_tc_weight_bytes": [_i, _i, _i, _i],
     "st2_convT_tc_weight_layout": [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp],
-    "st2_conv_transpose1d_tc": [C.POINTER(ConvArgs), _vp, _i, _i, _i, _i, _i, _vp],
     "st2_conv_transpose1d_tc2": [C.POINTER(ConvArgs), _vp, _i, _i, _i, _i, _i, _vp, _vp],
     "st2_conv_transpose1d": [C.POINTER(ConvArgs), _vp, _i, _i, _i, _i, _vp],
     "st2_instance_stats": [_vp, _ll, _i, _i, _i, _vp, _vp],

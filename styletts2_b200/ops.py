@@ -129,7 +129,6 @@ class _prof:
         return False
 
 
-CONVT_PHASE_MAJOR = os.environ.get("ST2_CONVT_PHASE_MAJOR", "1") != "0"   # tensor-core ConvTranspose through a phase-major scratch buffer
 USE_TC = os.environ.get("ST2_TC", "1") != "0"   # tensor-core (wgmma) conv path where a wtc buffer is given
 TC_MIN_WORK = 1 << 22                            # below this many MACs per utterance the SIMT kernel is used
 
@@ -236,11 +235,9 @@ def conv_transpose1d(x, wp, bias, *, K, stride, padding, pre_act=ACT_NONE, slope
     Lout = Lin * S + (1 if reflect_left1 else 0)
     if out is None:
         out = empty(B, Cout, Lout, device=x.device)
+    assert out.shape == (B, Cout, Lout) and out.stride(2) == 1 and out.stride(1) == Lout
     use_tc = wtc is not None and USE_TC
-    phase_major = use_tc and CONVT_PHASE_MAJOR and out.stride(2) == 1 and out.stride(1) == Lout
-    if use_tc and not phase_major and (wtc.mode & TC_TMAJOR):
-        use_tc = False   # the direct (strided-store) variant has no time-major kernel: FP32-pipe path
-    nparts = 1 if phase_major else S * (tc_stats_parts(Lin) if use_tc else stats_parts(Lin))
+    nparts = 1 if use_tc else S * stats_parts(Lin)
     stats = empty(B, Cout, nparts, 3, device=x.device) if want_stats else None
     a = ConvArgs()
     _fill_conv_args(a, x, wp, bias, out, K=1, stride=1, dil=1, pad=0, Lq=Lin, y_len=Lout, pre=None, pre_act=pre_act,
@@ -251,12 +248,9 @@ def conv_transpose1d(x, wp, bias, *, K, stride, padding, pre_act=ACT_NONE, slope
     flops = 2.0 * B * Cin * Cout * J * S * Lin
     if use_tc:
         with _prof(f"convT_tc m{wtc.mode} ci{Cin} co{Cout} k{K} s{S} L{Lin} B{B}", flops, nbytes, 2 if (wtc.mode & 15) == TC_FAST else 3):
-            if phase_major:
-                tmp = empty(S * B * Cout * Lin, device=x.device)
-                L.call("st2_conv_transpose1d_tc2", C.byref(a), ptr(wtc.buf), wtc.mode, K, S, padding, 1 if reflect_left1 else 0, ptr(tmp),
-                       stream_ptr())
-            else:
-                L.call("st2_conv_transpose1d_tc", C.byref(a), ptr(wtc.buf), wtc.mode, K, S, padding, 1 if reflect_left1 else 0, stream_ptr())
+            tmp = empty(S * B * Cout * Lin, device=x.device)
+            L.call("st2_conv_transpose1d_tc2", C.byref(a), ptr(wtc.buf), wtc.mode, K, S, padding, 1 if reflect_left1 else 0, ptr(tmp),
+                   stream_ptr())
     else:
         with _prof(f"convT_simt ci{Cin} co{Cout} k{K} s{S} L{Lin} B{B}", flops, nbytes):
             L.call("st2_conv_transpose1d", C.byref(a), ptr(wp), K, S, padding, 1 if reflect_left1 else 0, stream_ptr())
