@@ -29,8 +29,9 @@
 //    every channel row (rows of odd length start at any 4-byte phase; the phase becomes a per-channel offset of the
 //    scalar shared-memory reads of the conversion), a ring of four blocks per SM.
 //  * D accumulators live in the registers of two consumer warpgroups (output channels 0-63 / 64-127 of the tile, 128 frames
-//    each: m64n128 MMAs); the epilogue works on the fragments and fuses bias, residual, MRF accumulation and the InstanceNorm
-//    partial statistics (count, mean, M2) exactly like the SIMT kernel.  A 128-frame tile writes two partials, one per
+//    each: m64n128 MMAs); the epilogue fuses bias, residual, MRF accumulation and the InstanceNorm partial statistics
+//    (count, mean, M2) exactly like the SIMT kernel.  Its global traffic goes through a shared-memory transpose (SM_SLOT,
+//    epi_rows: whole channel rows per warp), its statistics work on the fragments.  A 128-frame tile writes two partials, one per
 //    64 frames, so the statistics layout does not depend on the tile width.  Output positions are contiguous
 //    (y_tstride = 1, no reflection duplicate): a ConvTranspose1d runs its phases into phase-major scratch rows that
 //    convT_interleave_kernel interleaves (st2_conv_transpose1d_tc2).
@@ -118,12 +119,12 @@ constexpr int SM_COEF = SM_RAW + RAW_STAGES * RAW_BYTES;
 constexpr int SM_EPI = SM_COEF + 4 * CIN_PAD_MAX * 4;   // per-channel prologue coefficients of the current utterance (4 x 1120 floats)
 constexpr int TCT_NC_MAX = 128;                   // output channels of the time-major kernel, max
 constexpr int SM_SLOT = SM_EPI + 2 * 4 * TCT_NC_MAX * 4;   // time-major statistics scratch [2 warpgroups][4 warps][128 channels]
-// time-major epilogue slot: SLOT_Q float4 of folded accumulators per consumer thread; float4 q of consumer thread i lives at
-// (q * NUM_CONS + i) * 16 bytes (conflict-free), and a thread only ever reads back what it wrote itself.  The output
-// values are computed from here by a rolled loop: unrolled over the register fragments, they were ~4300 straight-line
-// instructions at NC = 128 (69 KB of code, run once per tile and so mostly from a cold instruction cache).
-constexpr int SLOT_Q = 8;
-constexpr int SM_BAR = SM_SLOT + SLOT_Q * NUM_CONS * 16;
+// Epilogue transpose slot: SLOT_FLOATS floats per consumer warpgroup, one slice of the tile's outputs as [channel][frame]
+// rows (64 channels x 64 frames time-major, 32 channels x 128 frames channel-major; slot_index).  The fragments go in, each
+// warp then owns whole channel rows, so that one load or store instruction covers 32 consecutive frames of one channel
+// (128 contiguous bytes) instead of 4 or 8 short runs of the wgmma fragment mapping.
+constexpr int SLOT_FLOATS = 4096;
+constexpr int SM_BAR = SM_SLOT + 2 * SLOT_FLOATS * 4;
 constexpr int SM_TOTAL = SM_BAR + 512;
 static_assert(RAW_CHUNKS % ST_PER_CH == 0 && NUM_STAGERS % 64 == 0 && NUM_STAGERS % CB == 0, "stager mappings");
 static_assert(RAW_CHUNKS * 4 >= RW_MAX + 3 && RAW_PITCH >= RAW_CHUNKS * 4 && (RAW_PITCH * 4) % 128 == 64, "raw window rows");
@@ -511,14 +512,73 @@ __device__ __forceinline__ float epi_combine(const st2_conv_args& a, float v, fl
   return val;
 }
 
-// The epilogues read the residual and MRF operands of a group of elements BEFORE they store any of them.  The compiler
-// may not move a load above a store through a pointer that could alias it, so loading each element's operands just before
-// its store pays one full memory latency per element (the consumer warps have nothing else to issue meanwhile).  An
-// element's operands are only ever read by the thread that writes it, so the values are the same.
+// The epilogues read the residual and MRF operands of a whole slice BEFORE they store any of it.  The compiler may not move
+// a load above a store through a pointer that could alias it, so loading each element's operands just before its store
+// pays one full memory latency per element (the consumer warps have nothing else to issue meanwhile).  An element's
+// operands are only ever read by the thread that writes it, so the values are the same.
 __device__ __forceinline__ void epi_load(const st2_conv_args& a, const float* rrow, const float* yp, int oidx, bool ok, float& res_v,
                                          float& y_old) {
   res_v = (rrow && ok) ? rrow[oidx >> a.res_shift] : 0.f;
   y_old = (a.accum_mode != 0 && ok) ? yp[oidx] : 0.f;
+}
+
+// Float index of (channel row r, frame fr) in a warpgroup's slot of rows `pitch` (64 or 128) frames long.  The XOR keeps both
+// views free of bank conflicts: a fragment-order access (one register of 32 lanes: g = lane / 4 picks bits 0-2 of the frame
+// or the channel, t4 = lane % 4 bits 1-2 of the other) lands on 32 distinct banks, and a row access (one channel, frames
+// l + 32 m) only permutes the frames inside their aligned group of 32.  tests/test_cpu_epilogue_slot.py restates it.
+__device__ __forceinline__ int slot_index(int r, int fr, int pitch) { return r * pitch + (fr ^ ((r & 1) | ((r & 6) << 2))); }
+
+// Consumer warpgroup barrier around the slot (named barrier 3 + wg, 128 threads).
+__device__ __forceinline__ void wg_bar(uint32_t id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// Row phase of the epilogue for one warp: slot rows r0 .. r0 + nr - 1 (output channels co0 + r), lane l handling frames
+// l + 32 m of each, in batches of RB rows (nr is a multiple of RB).  Every residual / MRF operand of a batch is loaded first
+// (epi_load), then each value is combined, stored to y at frame t0 + fr when it exists (channel < Cout, fr < nfr) and
+// written back to the slot (0 where it does not) for the statistics.  The slot holds the folded accumulators, still scaled
+// by 2^18.  The batch loop stays rolled: compact code (the epilogue runs once per tile, mostly from a cold instruction
+// cache), and one batch's operands are what the consumer's 128 registers hold next to the accumulators.
+template <int RB, int FPL>
+__device__ __forceinline__ void epi_rows(const st2_conv_args& a, float* xs, int pitch, int r0, int nr, int co0, int b, int t0, int nfr,
+                                         int lane) {
+  // row pointers advance by one row per channel; a row at or beyond Cout is never dereferenced (every access is under cok)
+  const long long ylen = a.y_len, rlen = a.res ? a.res_len : 0;   // no residual: rrow stays null
+  float* yrow = a.y + (long long)b * a.y_bstride + (long long)(co0 + r0) * ylen;
+  const float* rrow = a.res ? a.res + (long long)b * a.res_bstride + (long long)(co0 + r0) * rlen : nullptr;
+#pragma unroll 1
+  for (int k0 = 0; k0 < nr; k0 += RB) {
+    float res_v[RB][FPL], y_old[RB][FPL], bias[RB];
+#pragma unroll
+    for (int k = 0; k < RB; ++k) {
+      const int co = co0 + r0 + k0 + k;
+      const bool cok = co < a.Cout;
+      bias[k] = (a.bias && cok) ? __ldg(a.bias + co) : 0.f;
+#pragma unroll
+      for (int m = 0; m < FPL; ++m) {
+        const int fr = lane + 32 * m;
+        epi_load(a, rrow, yrow, t0 + fr, cok && fr < nfr, res_v[k][m], y_old[k][m]);
+      }
+      yrow += ylen;
+      rrow += rlen;
+    }
+    yrow -= RB * ylen;
+#pragma unroll
+    for (int k = 0; k < RB; ++k) {
+      const int r = r0 + k0 + k, sw = (r & 1) | ((r & 6) << 2);   // slot_index's swizzle of row r
+      const bool cok = co0 + r < a.Cout;
+      float* xr = xs + r * pitch;
+#pragma unroll
+      for (int m = 0; m < FPL; ++m) {
+        const int fr = lane + 32 * m;
+        float val = 0.f;
+        if (cok && fr < nfr) {
+          val = epi_combine(a, xr[fr ^ sw] * D_UNSCALE, bias[k], res_v[k][m], y_old[k][m]);
+          yrow[t0 + fr] = val;
+        }
+        xr[fr ^ sw] = val;
+      }
+      yrow += ylen;
+    }
+  }
 }
 
 template <int MODE>
@@ -563,62 +623,46 @@ conv1d_tc_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const int
       });
       wg_fence_regs(d0);
       if (MODE != MODE_X3) wg_fence_regs(d1);
-      // fold the correction accumulator: d0 holds the unscaled sums from here on (d1 is dead)
+      // fold the correction accumulator into d0 (d1 is dead from here on)
 #pragma unroll
       for (int r = 0; r < 64; ++r) {
         float v = d0[r];
         if (MODE == MODE_ACC) v = fmaf(d1[r], ACC_LO_UNSCALE, v);
         if (MODE == MODE_FAST) v += d1[r];
-        d0[r] = v * D_UNSCALE;
+        d0[r] = v;
       }
 
-      // ---- epilogue: row = output channel, column = frame; each 64-frame half of the tile (fragment columns j = 8 h ..
-      // 8 h + 7) is one statistics partial.  The second half of a tail tile can lie entirely beyond Lq: no partial then.
-      float* yb = a.y + (long long)tc_.b * a.y_bstride;
-      const float* rbase = a.res ? a.res + (long long)tc_.b * a.res_bstride : nullptr;
-      float biases[2];
+      // ---- epilogue: row = output channel, column = frame.  Each 64-frame half h of the tile (fragment columns j = 8 h ..
+      // 8 h + 7) is one slice through the warpgroup's slot and one statistics partial: fragment float 4 (8 h + j) + 2 i + c
+      // is channel w * 16 + g + 8 i, frame 8 j + 2 t4 + c of the half.  Each warp computes 16 whole channel rows (epi_rows),
+      // the values come back into the fragments, and the half's statistics follow.  The second half of a tail tile can lie
+      // entirely beyond Lq: no partial then.
+      float* xs = reinterpret_cast<float*>(smem + SM_SLOT) + wg * SLOT_FLOATS;
+      const uint32_t bar_id = 3 + wg;
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
-        biases[i] = (a.bias && co < a.Cout) ? a.bias[co] : 0.f;
-      }
+      for (int h = 0; h < TN / TP; ++h) {
+        const int t0 = tc_.tq * TN + h * TP;
+        wg_bar(bar_id);   // the previous half's (or tile's) readers are done
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
-        const bool cok = co < a.Cout;
-        const float bias = biases[i];
-        float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-        const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
+        for (int q = 0; q < 32; ++q) xs[slot_index(w * 16 + g + 8 * ((q >> 1) & 1), 8 * (q >> 2) + 2 * t4 + (q & 1), TP)] = d0[32 * h + q];
+        wg_bar(bar_id);
+        epi_rows<8, TP / 32>(a, xs, TP, w * 16, 16, tc_.cob * TM + wg * 64, tc_.b, t0, a.Lq - t0, lane);
+        wg_bar(bar_id);
 #pragma unroll
-        for (int h = 0; h < TN / TP; ++h) {
-          const int t0 = tc_.tq * TN + h * TP;
-          const int ncols = min(TP, a.Lq - t0);
+        for (int q = 0; q < 32; ++q) d0[32 * h + q] = xs[slot_index(w * 16 + g + 8 * ((q >> 1) & 1), 8 * (q >> 2) + 2 * t4 + (q & 1), TP)];
+        const int ncols = min(TP, a.Lq - t0);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int co = tc_.cob * TM + wg * 64 + w * 16 + g + 8 * i;
+          const bool cok = co < a.Cout;
           float s = 0.f, n = 0.f;
 #pragma unroll
-          for (int j0 = 0; j0 < 8; j0 += 4) {
-            float res_v[8], y_old[8];   // 8 elements of this row: operands first, then the stores (epi_load)
+          for (int j = 0; j < 8; ++j) {
 #pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                const int col = 8 * (j0 + jj) + 2 * t4 + c;
-                epi_load(a, rrow, yp, t0 + col, cok && col < ncols, res_v[2 * jj + c], y_old[2 * jj + c]);
-              }
-            }
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                const int j = j0 + jj;
-                const int r = 4 * (8 * h + j) + 2 * i + c, col = 8 * j + 2 * t4 + c;
-                float val = 0.f;
-                if (cok && col < ncols) {
-                  val = epi_combine(a, d0[r], bias, res_v[2 * jj + c], y_old[2 * jj + c]);
-                  yp[t0 + col] = val;
-                  s += val;
-                  n += 1.f;
-                }
-                d0[r] = val;
+            for (int c = 0; c < 2; ++c) {
+              if (cok && 8 * j + 2 * t4 + c < ncols) {
+                s += d0[4 * (8 * h + j) + 2 * i + c];
+                n += 1.f;
               }
             }
           }
@@ -701,7 +745,13 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
     const bool leader = (tid & 127) == 0;
     const uint32_t lbo_x = (uint32_t)RWP * 16, lbo_w = (uint32_t)NC * 16;
     float* red = reinterpret_cast<float*>(smem + SM_EPI) + wg * 4 * TCT_NC_MAX;   // [4 warps][TCT_NC_MAX channels]
-    float4* slot = reinterpret_cast<float4*>(smem + SM_SLOT) + tid;              // this thread's float4 q at slot[q * NUM_CONS]
+    float* xs = reinterpret_cast<float*>(smem + SM_SLOT) + wg * SLOT_FLOATS;
+    const uint32_t bar_id = 3 + wg;
+    // fragment float 4 j + q (frame w * 16 + g + 8 (q >> 1) of channel 8 j + 2 t4 + (q & 1)) sits at slot float
+    // fofs[q] + 8 TP (j - c0 / 8) of the slice starting at channel c0: the swizzle of a row does not depend on j
+    int fofs[4];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) fofs[q] = slot_index(2 * t4 + (q & 1), w * 16 + g + 4 * (q & 2), TP);
     ConsumerRing ring;
     for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
       const int tq = tile % n_tq, b = tile / n_tq;
@@ -723,74 +773,28 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
       // second warpgroup of a tail tile can lie entirely beyond Lq (ncols <= 0): it then writes nothing.
       const int t0 = tq * TN + wg * TP;
       const int ncols = min(TP, a.Lq - t0);
-      float* yb = a.y + (long long)b * a.y_bstride;
-      const float* rbase = a.res ? a.res + (long long)b * a.res_bstride : nullptr;
-      // residual / MRF operands of channel group j, loaded one group ahead of its stores (epi_load)
-      float res_n[4], old_n[4];
-      auto load_group = [&](int j) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int co = 8 * j + 2 * t4 + c;
-          const bool cok = co < a.Cout;
-          const float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-          const float* rrow = rbase ? rbase + (long long)(cok ? co : 0) * a.res_len : nullptr;
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            const int fr = w * 16 + g + 8 * i;
-            epi_load(a, rrow, yp, t0 + fr, cok && fr < ncols, res_n[2 * i + c], old_n[2 * i + c]);
-          }
-        }
-      };
-      // Output values, SLOT_Q channel groups at a time through the slot: float4 j - j0 holds frames w * 16 + g + {0, 8} (i)
-      // of channels 8 j + 2 t4 + {0, 1} (c) as components 2 i + c.  The loop over the groups stays rolled (compact code,
-      // see SM_SLOT); the values come back into the fragments for the statistics.
-#pragma unroll
-      for (int j0 = 0; j0 < NJ; j0 += SLOT_Q) {
-        constexpr int NQ = NJ < SLOT_Q ? NJ : SLOT_Q;   // NJ is 2, 4, 8, 12 or 16
-        const int nq = min(NQ, NJ - j0);
-#pragma unroll
-        for (int q = 0; q < NQ; ++q)
-          if (q < nq) slot[q * NUM_CONS] = make_float4(d[4 * (j0 + q)], d[4 * (j0 + q) + 1], d[4 * (j0 + q) + 2], d[4 * (j0 + q) + 3]);
-        load_group(j0);
-        auto value_group = [&](int j) {
-          float res_v[4], y_old[4];
-#pragma unroll
-          for (int k = 0; k < 4; ++k) { res_v[k] = res_n[k]; y_old[k] = old_n[k]; }
-          if (j + 1 < j0 + nq) load_group(j + 1);
-          const float4 qv = slot[(j - j0) * NUM_CONS];
-          const float v[4] = {qv.x, qv.y, qv.z, qv.w};
-          float o[4];
-#pragma unroll
-          for (int c = 0; c < 2; ++c) {
-            const int co = 8 * j + 2 * t4 + c;
-            const bool cok = co < a.Cout;
-            float* yp = yb + (long long)(cok ? co : 0) * a.y_len;
-            const float bias = (a.bias && cok) ? __ldg(a.bias + co) : 0.f;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              const int fr = w * 16 + g + 8 * i;
-              float val = 0.f;
-              if (cok && fr < ncols) {
-                val = epi_combine(a, v[2 * i + c] * D_UNSCALE, bias, res_v[2 * i + c], y_old[2 * i + c]);
-                yp[t0 + fr] = val;
-              }
-              o[2 * i + c] = val;
-            }
-          }
-          slot[(j - j0) * NUM_CONS] = make_float4(o[0], o[1], o[2], o[3]);
-        };
-        if constexpr (NJ > 4) {
+      // Output values through the warpgroup's slot in slices of up to 64 channels: fragment float 4 j + 2 i + c is frame
+      // w * 16 + g + 8 i of channel 8 j + 2 t4 + c.  Each warp computes a quarter of the slice's channel rows (epi_rows); the
+      // values come back into the fragments for the statistics.
+      constexpr int SC = NC < 64 ? NC : 64;
 #pragma unroll 1
-          for (int j = j0; j < j0 + nq; ++j) value_group(j);
-        } else {   // NC <= 32: short enough unrolled (rolled, ptxas spills in the stager warps of NC = 32)
+      for (int c0 = 0; c0 < NC; c0 += SC) {
+        wg_bar(bar_id);   // the previous slice's (or tile's) readers are done
 #pragma unroll
-          for (int j = j0; j < j0 + nq; ++j) value_group(j);
-        }
+        for (int j = 0; j < NJ; ++j)
+          if (8 * j >= c0 && 8 * j < c0 + SC) {
 #pragma unroll
-        for (int q = 0; q < NQ; ++q)
-          if (q < nq) {
-            const float4 qv = slot[q * NUM_CONS];
-            d[4 * (j0 + q)] = qv.x; d[4 * (j0 + q) + 1] = qv.y; d[4 * (j0 + q) + 2] = qv.z; d[4 * (j0 + q) + 3] = qv.w;
+            for (int q = 0; q < 4; ++q) xs[fofs[q] - TP * c0 + 8 * TP * j] = d[4 * j + q];
+          }
+        wg_bar(bar_id);
+        const int nr = min(SC, NC - c0) / 4;
+        epi_rows<(SC < 32 ? SC / 4 : 8), TP / 32>(a, xs, TP, w * nr, nr, c0, b, t0, ncols, lane);
+        wg_bar(bar_id);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j)
+          if (8 * j >= c0 && 8 * j < c0 + SC) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) d[4 * j + q] = xs[fofs[q] - TP * c0 + 8 * TP * j];
           }
       }
       // per-thread sums of each channel over its two frames, in the order the values were produced
@@ -807,7 +811,6 @@ conv1d_tct_kernel(const st2_conv_args a, const uint4* __restrict__ wtc, const in
           s[2 * j + c] = ss;
         }
       if (a.stats && ncols > 0) {
-        const uint32_t bar_id = 3 + wg;
         // pass 1: sums over the 16 frames of the warp (lanes with equal t4), then over the warpgroup's four warps
 #pragma unroll
         for (int k = 0; k < 2 * NJ; ++k) {
